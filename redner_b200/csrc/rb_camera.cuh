@@ -29,13 +29,7 @@ RB_HD D2 d2(double x, double y) { D2 r; r.x = x; r.y = y; return r; }
 
 // ---- Brown-Conrady lens distortion on normalised screen coordinates (src/camera_distortion.h) ----
 // distort: undistorted -> distorted position; optional forward-mode rows d(out.x)/d(pos), d(out.y)/d(pos).
-// (Bodies behind RB_COLD, see rb_math.cuh.)
-RB_COLD D2 cam_distort_impl(const DevCamera& cam, D2 pos, D2* dx_dpos, D2* dy_dpos);
-RB_HD D2 cam_distort(const DevCamera& cam, D2 pos, D2* dx_dpos = nullptr, D2* dy_dpos = nullptr) {
-    if (!RB_CAM_DISTORT(cam)) return pos;
-    return cam_distort_impl(cam, pos, dx_dpos, dy_dpos);
-}
-RB_COLD D2 cam_distort_impl(const DevCamera& cam, D2 pos, D2* dx_dpos, D2* dy_dpos) {
+RB_HD D2 cam_distort_impl(const DevCamera& cam, D2 pos, D2* dx_dpos, D2* dy_dpos) {
     const double* k = cam.distortion;
     const double p0 = k[6], p1 = k[7];
     double x = 2.0 * (pos.x - 0.5), y = 2.0 * (pos.y - 0.5);
@@ -59,16 +53,12 @@ RB_COLD D2 cam_distort_impl(const DevCamera& cam, D2 pos, D2* dx_dpos, D2* dy_dp
     }
     return d2((xx + 1) / 2, (yy + 1) / 2);
 }
-// Adjoint of cam_distort; d_params (8 doubles, may be null) receives the parameter gradient.
-RB_COLD void d_cam_distort_impl(const DevCamera& cam, D2 pos, D2 d_out, double* d_params, D2& d_pos);
-RB_HD void d_cam_distort(const DevCamera& cam, D2 pos, D2 d_out, double* d_params, D2& d_pos) {
-    if (!RB_CAM_DISTORT(cam)) {
-        d_pos = d_out; // (assignment, as in the reference :96-99)
-        return;
-    }
-    d_cam_distort_impl(cam, pos, d_out, d_params, d_pos);
+RB_HD D2 cam_distort(const DevCamera& cam, D2 pos, D2* dx_dpos = nullptr, D2* dy_dpos = nullptr) {
+    if (!RB_CAM_DISTORT(cam)) return pos;
+    return cam_distort_impl(cam, pos, dx_dpos, dy_dpos);
 }
-RB_COLD void d_cam_distort_impl(const DevCamera& cam, D2 pos, D2 d_out, double* d_params, D2& d_pos) {
+// Adjoint of cam_distort; d_params (8 doubles, may be null) receives the parameter gradient.
+RB_HD void d_cam_distort_impl(const DevCamera& cam, D2 pos, D2 d_out, double* d_params, D2& d_pos) {
     const double* k = cam.distortion;
     const double p0 = k[6], p1 = k[7];
     double x = 2.0 * (pos.x - 0.5), y = 2.0 * (pos.y - 0.5);
@@ -107,13 +97,15 @@ RB_COLD void d_cam_distort_impl(const DevCamera& cam, D2 pos, D2 d_out, double* 
         d_params[7] += d_p[1];
     }
 }
-// distorted -> undistorted position by Gauss-Newton (src/camera_distortion.h:171-198)
-RB_COLD D2 cam_inverse_distort_impl(const DevCamera& cam, D2 pos);
-RB_HD D2 cam_inverse_distort(const DevCamera& cam, D2 pos) {
-    if (!RB_CAM_DISTORT(cam)) return pos;
-    return cam_inverse_distort_impl(cam, pos);
+RB_HD void d_cam_distort(const DevCamera& cam, D2 pos, D2 d_out, double* d_params, D2& d_pos) {
+    if (!RB_CAM_DISTORT(cam)) {
+        d_pos = d_out; // (assignment, as in the reference :96-99)
+        return;
+    }
+    d_cam_distort_impl(cam, pos, d_out, d_params, d_pos);
 }
-RB_COLD D2 cam_inverse_distort_impl(const DevCamera& cam, D2 pos) {
+// distorted -> undistorted position by Gauss-Newton (src/camera_distortion.h:171-198)
+RB_HD D2 cam_inverse_distort_impl(const DevCamera& cam, D2 pos) {
     D2 result = pos;
     double err = 0;
     int iter = 0;
@@ -127,16 +119,12 @@ RB_COLD D2 cam_inverse_distort_impl(const DevCamera& cam, D2 pos) {
     } while (err > 1e-3 && iter++ < 1000);
     return result;
 }
-// Adjoint through the implicit function theorem (src/camera_distortion.h:200-258)
-RB_COLD void d_cam_inverse_distort_impl(const DevCamera& cam, D2 pos, D2 d_out, double* d_params, D2& d_pos);
-RB_HD void d_cam_inverse_distort(const DevCamera& cam, D2 pos, D2 d_out, double* d_params, D2& d_pos) {
-    if (!RB_CAM_DISTORT(cam)) {
-        d_pos = d_out;
-        return;
-    }
-    d_cam_inverse_distort_impl(cam, pos, d_out, d_params, d_pos);
+RB_HD D2 cam_inverse_distort(const DevCamera& cam, D2 pos) {
+    if (!RB_CAM_DISTORT(cam)) return pos;
+    return cam_inverse_distort_impl(cam, pos);
 }
-RB_COLD void d_cam_inverse_distort_impl(const DevCamera& cam, D2 pos, D2 d_out, double* d_params, D2& d_pos) {
+// Adjoint through the implicit function theorem (src/camera_distortion.h:200-258)
+RB_HD void d_cam_inverse_distort_impl(const DevCamera& cam, D2 pos, D2 d_out, double* d_params, D2& d_pos) {
     D2 result = cam_inverse_distort(cam, pos);
     D2 fx, fy;
     cam_distort(cam, result, &fx, &fy);
@@ -147,8 +135,15 @@ RB_COLD void d_cam_inverse_distort_impl(const DevCamera& cam, D2 pos, D2 d_out, 
     d_pos.x -= d_result.x;
     d_pos.y -= d_result.y;
 }
+RB_HD void d_cam_inverse_distort(const DevCamera& cam, D2 pos, D2 d_out, double* d_params, D2& d_pos) {
+    if (!RB_CAM_DISTORT(cam)) {
+        d_pos = d_out;
+        return;
+    }
+    d_cam_inverse_distort_impl(cam, pos, d_out, d_params, d_pos);
+}
 
-RB_COLD void cam_sample_primary_any(const DevCamera& cam, double sx_, double sy_, D3& org, D3& dir) {
+RB_HD void cam_sample_primary_any(const DevCamera& cam, double sx_, double sy_, D3& org, D3& dir) {
     D2 undist = cam_inverse_distort(cam, d2(sx_, sy_)); // (identity without a lens model)
     const double sx = undist.x, sy = undist.y;
     const double* C = cam.c2w;
@@ -290,7 +285,7 @@ struct CamAcc {
 
 // Adjoint of cam_sample_primary w.r.t. camera parameters (screen-position gradients are only needed for
 // distortion / screen_gradient_image; the latter is accumulated by the caller through d_screen).
-RB_COLD_D void d_cam_sample_primary_any(const DevCamera& cam, Real sx_, Real sy_, const DRay& d_ray, CamAcc& acc, V2* d_screen_out) {
+RB_D void d_cam_sample_primary_any(const DevCamera& cam, Real sx_, Real sy_, const DRay& d_ray, CamAcc& acc, V2* d_screen_out) {
     // With a lens model the ray is generated at the UNDISTORTED position and the adjoint w.r.t. that position flows back
     // through inverse_distort (parameters + original position), src/camera.h:205-206,262-277.
     const D2 spos = d2(sx_, sy_);
@@ -461,24 +456,7 @@ RB_HD bool cam_project(const DevCamera& cam, V3 p0, V3 p1, V2& pp0, V2& pp1) {
     pp1 = cam_to_screen(cam, b);
     return true;
 }
-RB_COLD_D void d_cam_to_screen_any(const DevCamera& cam, V3 pt, Real dx, Real dy, CamAcc& acc, V3& d_pt);
-RB_D void d_cam_to_screen(const DevCamera& cam, V3 pt, Real dx, Real dy, CamAcc& acc, V3& d_pt) {
-    if (RB_CAM_GENERAL(cam)) {
-        d_cam_to_screen_any(cam, pt, dx, dy, acc, d_pt);
-        return;
-    }
-    M3 K = cam_m3(cam.intr);
-    Real aspect = Real(cam.width) / Real(cam.height);
-    V3 ip = mul(K, pt);
-    M3 d_K = zero_m3();
-    V2 q = mk2(ip.x / ip.z, ip.y / ip.z);
-    V2 d_q = mk2(dx * Real(0.5), dy * Real(-0.5) * aspect);
-    V3 d_ip = mk3(d_q.x / ip.z, d_q.y / ip.z, -(d_q.x * q.x / ip.z + d_q.y * q.y / ip.z));
-    d_outer_acc(d_K, d_ip, pt);
-    acc.add_intr(d_K);
-    d_pt += mul_t(d_ip, K);
-}
-RB_COLD_D void d_cam_to_screen_any(const DevCamera& cam, V3 pt, Real dx, Real dy, CamAcc& acc, V3& d_pt) {
+RB_D void d_cam_to_screen_any(const DevCamera& cam, V3 pt, Real dx, Real dy, CamAcc& acc, V3& d_pt) {
     if (RB_CAM_DISTORT(cam)) { // adjoint of the final distort(): parameters, and the undistorted position for the rest
         V2 q = cam_to_screen_undistorted(cam, pt);
         double d_par[8] = {0, 0, 0, 0, 0, 0, 0, 0};
@@ -516,6 +494,22 @@ RB_COLD_D void d_cam_to_screen_any(const DevCamera& cam, V3 pt, Real dx, Real dy
     } else {
         d_ip = mk3(dx * Real(0.5), dy * Real(-0.5) * aspect, 0);
     }
+    d_outer_acc(d_K, d_ip, pt);
+    acc.add_intr(d_K);
+    d_pt += mul_t(d_ip, K);
+}
+RB_D void d_cam_to_screen(const DevCamera& cam, V3 pt, Real dx, Real dy, CamAcc& acc, V3& d_pt) {
+    if (RB_CAM_GENERAL(cam)) {
+        d_cam_to_screen_any(cam, pt, dx, dy, acc, d_pt);
+        return;
+    }
+    M3 K = cam_m3(cam.intr);
+    Real aspect = Real(cam.width) / Real(cam.height);
+    V3 ip = mul(K, pt);
+    M3 d_K = zero_m3();
+    V2 q = mk2(ip.x / ip.z, ip.y / ip.z);
+    V2 d_q = mk2(dx * Real(0.5), dy * Real(-0.5) * aspect);
+    V3 d_ip = mk3(d_q.x / ip.z, d_q.y / ip.z, -(d_q.x * q.x / ip.z + d_q.y * q.y / ip.z));
     d_outer_acc(d_K, d_ip, pt);
     acc.add_intr(d_K);
     d_pt += mul_t(d_ip, K);

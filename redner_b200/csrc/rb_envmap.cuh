@@ -33,7 +33,7 @@ RB_HD EnvUV envmap_uv(const DevEnvmap& e, V3 local_dir, const RayDiff& rd, bool 
     }
     return r;
 }
-RB_COLD V3 envmap_eval(const DevEnvmap& e, V3 dir, const RayDiff& rd) {
+RB_HD V3 envmap_eval(const DevEnvmap& e, V3 dir, const RayDiff& rd) {
     V3 local_dir = normalize(env_xfm_vector(e.w2e, dir));
     EnvUV q = envmap_uv(e, local_dir, rd, local_dir.y < 1); // singular at (0, 1, 0): unfiltered there
     Real o[3];
@@ -41,7 +41,7 @@ RB_COLD V3 envmap_eval(const DevEnvmap& e, V3 dir, const RayDiff& rd) {
     return mk3(o[0], o[1], o[2]);
 }
 // d_values: gradient texture; d_w2e: 16 floats (row-major 4x4) accumulated with aggregated atomics
-RB_COLD_D void d_envmap_eval(const DevEnvmap& e, V3 dir, const RayDiff& rd, V3 d_out, const rb_texture& d_values, float* d_w2e, V3& d_dir, RayDiff& d_rd) {
+RB_D void d_envmap_eval(const DevEnvmap& e, V3 dir, const RayDiff& rd, V3 d_out, const rb_texture& d_values, float* d_w2e, V3& d_dir, RayDiff& d_rd) {
     V3 n_local = env_xfm_vector(e.w2e, dir);
     V3 l = normalize(n_local);
     EnvUV q = envmap_uv(e, l, rd, true); // (the adjoint always differentiates the filtered branch, src/envmap.h:118-130)
@@ -96,7 +96,7 @@ RB_HD int env_cdf_pick(const float* cdf, int n, double x) {
     }
     return rb_clampi(lo - 1, 0, n - 1);
 }
-RB_COLD V3 envmap_sample(const DevEnvmap& e, double sx, double sy) {
+RB_HD V3 envmap_sample(const DevEnvmap& e, double sx, double sy) {
     int w = e.values.width[0], h = e.values.height[0];
     int yp = env_cdf_pick(e.cdf_ys, h, sy);
     sy = yp < h - 1 ? (sy - e.cdf_ys[yp]) / ((double)e.cdf_ys[yp + 1] - e.cdf_ys[yp]) : (sy - e.cdf_ys[yp]) / (1 - (double)e.cdf_ys[yp]);
@@ -111,7 +111,7 @@ RB_COLD V3 envmap_sample(const DevEnvmap& e, double sx, double sy) {
     V3 local = mk3((Real)(sp * st), (Real)ct, (Real)(-cp * st));
     return env_xfm_vector(e.e2w, local);
 }
-RB_COLD Real envmap_pdf(const DevEnvmap& e, V3 dir) {
+RB_HD Real envmap_pdf(const DevEnvmap& e, V3 dir) {
     V3 l = env_xfm_vector(e.w2e, dir);
     V2 uv = mk2(atan2(l.x, -l.z) / Real(2 * RB_PI), env_safe_acos(l.y) / Real(RB_PI));
     int w = e.values.width[0], h = e.values.height[0];

@@ -26,7 +26,7 @@
 #include <string>
 #include <vector>
 
-#include "rb_lean_api.h"
+#include "rb_kernel_set.h"
 #include "rb_render.cuh"
 #include "rb_scene.cuh"
 
@@ -143,10 +143,11 @@ extern "C" int rb_render(const rb_scene* scene_, const rb_options* opt, float* i
         }
     }
     rp.only_radiance = only_radiance ? 1 : 0;
-    // The feature-free instantiation of the kernels (rb_kernels_lean.cu) serves the common configuration.
+    // The feature-free instantiation of the kernels (rb_kernels_lean.cu) serves the common configuration; `kern` holds the kernels of
+    // the chosen instantiation, and every launch of one of them below goes through it.
     const bool lean_allowed = getenv("RB_NO_LEAN") == nullptr; // (test hook: force the general kernels)
     const bool lean = lean_allowed && only_radiance && !scene->dev.has_envmap && scene->dev.cam.type == RB_CAMERA_PERSPECTIVE && !scene->dev.cam.has_distortion;
-    namespace la = rb_lean_api;
+    const RenderKernels kern = lean ? rb_lean::render_kernels() : render_kernels();
     rp.nd = rb_compute_num_channels(opt->channels, opt->num_channels, rp.max_generic);
     rp.rad_off = -1;
     for (int i = 0, off = 0; i < opt->num_channels; i++) {
@@ -192,15 +193,12 @@ std::vector<cudaEvent_t>& ev = events.ev;
     std::vector<BandCounters> host_counters;
     long long num_bands_done = 0;
     std::unique_lock<std::mutex> scratch_lock; // per-device scratch, held for the backward pass (released before the guard runs)
+    void* args[] = {&scene->dev, &ka}; // parameters of every kernel in `kern` but the primary-edge pair (read at each launch)
     RB_CUDA_OK(cudaEventRecord(ev[0], stream));
     if (image != nullptr) {
         if (only_radiance) {
-            if (lean) {
-                la::forward(&scene->dev, &ka, la::grid(la::K_FORWARD, scene->device), stream);
-            } else {
-                int grid = pick_grid((const void*)k_forward, scene->device, RB_BLOCK_FWD);
-                k_forward<<<grid, RB_BLOCK_FWD, 0, stream>>>(scene->dev, ka);
-            }
+            int grid = pick_grid(kern.forward, scene->device, RB_BLOCK_FWD);
+            RB_CUDA_OK(cudaLaunchKernel(kern.forward, grid, RB_BLOCK_FWD, args, 0, stream));
         } else {
             int grid = pick_grid((const void*)k_forward_channels, scene->device);
             k_forward_channels<<<grid, RB_BLOCK, 0, stream>>>(scene->dev, ka);
@@ -321,22 +319,10 @@ std::vector<cudaEvent_t>& ev = events.ev;
         ka.edge_hist = (unsigned*)(scratch + o_hist);
         ka.edge_offs = (unsigned*)(scratch + o_eoffs);
         ka.edge_cursor = (unsigned*)(scratch + o_ecur);
-        // Persistent-warp hierarchy pick (k_bwd_sec_pick_hier: resumable walks, finished lanes refilled from a work counter): identical
-        // picks, but slower than the plain kernel on C2 and the teapot: the stage waits on dependent loads, not on issue slots, so
-        // idle lanes cost nothing and the refill logic is pure overhead.  Opt-in for measurements.
-        ka.hier_persistent = getenv("RB_PERSISTENT_PICK") != nullptr ? 1 : 0;
-        int grid_t, grid_p, grid_s, grid_w;
-        if (lean) {
-            grid_t = la::grid(la::K_BWD_TRACE, scene->device);
-            grid_p = la::grid(la::K_BWD_SEC_PICK, scene->device);
-            grid_s = la::grid(la::K_BWD_SEC_SHADE, scene->device);
-            grid_w = la::grid(la::K_BWD_SWEEP, scene->device);
-        } else {
-            grid_t = pick_grid((const void*)k_bwd_trace, scene->device, RB_BLOCK_TRACE);
-            grid_p = pick_grid((const void*)k_bwd_sec_pick, scene->device, RB_BLOCK_SEC);
-            grid_s = pick_grid((const void*)k_bwd_sec_shade, scene->device, RB_BLOCK_SEC);
-            grid_w = pick_grid((const void*)k_bwd_sweep, scene->device, RB_BLOCK_SWEEP, RB_SMEM_CAM(RB_BLOCK_SWEEP));
-        }
+        const int grid_t = pick_grid(kern.bwd_trace, scene->device, RB_BLOCK_TRACE);
+        const int grid_p = pick_grid(kern.bwd_sec_pick, scene->device, RB_BLOCK_SEC);
+        const int grid_s = pick_grid(kern.bwd_sec_shade, scene->device, RB_BLOCK_SEC);
+        const int grid_w = pick_grid(kern.bwd_sweep, scene->device, RB_BLOCK_SWEEP, RB_SMEM_CAM(RB_BLOCK_SWEEP));
         long long band_idx = 0;
         for (long long i0 = 0; i0 < total_samples; i0 += band, band_idx++) {
             ka.band_i0 = i0;
@@ -344,8 +330,7 @@ std::vector<cudaEvent_t>& ev = events.ev;
             ka.counters = counters + band_idx;
             cudaEvent_t* e4 = &events.ev[(size_t)(5 + 4 * band_idx)];
             RB_CUDA_OK(cudaEventRecord(e4[0], stream));
-            if (lean) la::bwd_trace(&scene->dev, &ka, grid_t, stream);
-            else k_bwd_trace<<<grid_t, RB_BLOCK_TRACE, 0, stream>>>(scene->dev, ka);
+            RB_CUDA_OK(cudaLaunchKernel(kern.bwd_trace, grid_t, RB_BLOCK_TRACE, args, 0, stream));
             RB_CUDA_OK(cudaEventRecord(e4[1], stream));
             {
                 auto counts = thrust::make_transform_iterator(thrust::counting_iterator<int>(0), ListCountOf{ka.nrec, secondary ? ka.vmask : nullptr});
@@ -354,22 +339,14 @@ std::vector<cudaEvent_t>& ev = events.ev;
             }
             launches += 4;
             if (secondary) {
-                if (lean) la::bwd_sec_pick(&scene->dev, &ka, grid_p, stream);
-                else k_bwd_sec_pick<<<grid_p, RB_BLOCK_SEC, 0, stream>>>(scene->dev, ka);
-                if (ka.hier_persistent) {
-                    if (lean) la::bwd_sec_pick_hier(&scene->dev, &ka, grid_p, stream);
-                    else k_bwd_sec_pick_hier<<<grid_p, RB_BLOCK_SEC, 0, stream>>>(scene->dev, ka);
-                    launches++;
-                }
+                RB_CUDA_OK(cudaLaunchKernel(kern.bwd_sec_pick, grid_p, RB_BLOCK_SEC, args, 0, stream));
                 k_sec_offsets<<<1, 1024, 0, stream>>>(ka, scene->dev.num_edges);
                 k_sec_scatter<<<sms * 8, 256, 0, stream>>>(ka);
-                if (lean) la::bwd_sec_shade(&scene->dev, &ka, grid_s, stream);
-                else k_bwd_sec_shade<<<grid_s, RB_BLOCK_SEC, 0, stream>>>(scene->dev, ka);
+                RB_CUDA_OK(cudaLaunchKernel(kern.bwd_sec_shade, grid_s, RB_BLOCK_SEC, args, 0, stream));
                 launches += 4;
             }
             RB_CUDA_OK(cudaEventRecord(e4[2], stream));
-            if (lean) la::bwd_sweep(&scene->dev, &ka, grid_w, stream);
-            else k_bwd_sweep<<<grid_w, RB_BLOCK_SWEEP, RB_SMEM_CAM(RB_BLOCK_SWEEP), stream>>>(scene->dev, ka);
+            RB_CUDA_OK(cudaLaunchKernel(kern.bwd_sweep, grid_w, RB_BLOCK_SWEEP, args, RB_SMEM_CAM(RB_BLOCK_SWEEP), stream));
             launches++;
             RB_CUDA_OK(cudaEventRecord(e4[3], stream));
         }
@@ -380,7 +357,7 @@ std::vector<cudaEvent_t>& ev = events.ev;
         }
         RB_CUDA_OK(cudaEventRecord(ev[2], stream));
         if (scene->dev.use_primary_edge && scene->dev.num_edges > 0 && scene->dev.prim_edge_cdf != nullptr) {
-            int grid_e = lean ? la::grid(la::K_PRIMARY_EDGE, scene->device) : pick_grid((const void*)k_primary_edge, scene->device, RB_BLOCK_PRIM, RB_SMEM_CAM(RB_BLOCK_PRIM));
+            int grid_e = pick_grid(kern.primary_edge, scene->device, RB_BLOCK_PRIM, RB_SMEM_CAM(RB_BLOCK_PRIM));
             int dim_base = primary_edge_dim_base(scene->dev, rp);
             unsigned *k0 = (unsigned*)(scratch + o_k0), *k1 = (unsigned*)(scratch + o_k1), *v0 = (unsigned*)(scratch + o_v0), *v1 = (unsigned*)(scratch + o_v1);
             int ebits = 1;
@@ -388,13 +365,13 @@ std::vector<cudaEvent_t>& ev = events.ev;
             for (long long t0 = 0; t0 < total_e; t0 += band_e) {
                 int n = (int)std::min<long long>(band_e, total_e - t0);
                 int grid_k = std::min((n + 255) / 256, sms * 16);
-                if (lean) la::prim_keys(&scene->dev, &ka, dim_base, t0, n, k0, v0, grid_k, stream);
-                else k_prim_keys<<<grid_k, 256, 0, stream>>>(scene->dev, ka, dim_base, t0, n, k0, v0);
+                void* key_args[] = {&scene->dev, &ka, &dim_base, &t0, &n, &k0, &v0};
+                RB_CUDA_OK(cudaLaunchKernel(kern.prim_keys, grid_k, 256, key_args, 0, stream));
                 // sort on the edge bits and the top 8 bits of the position only (coarser order is enough for coherence)
                 int lo = std::max(0, 31 - ebits - 8);
                 cub::DeviceRadixSort::SortPairs(scratch + o_sort, sort_bytes, k0, k1, v0, v1, n, lo, 32, stream);
-                if (lean) la::primary_edge(&scene->dev, &ka, dim_base, t0, n, k1, v1, grid_e, stream);
-                else k_primary_edge<<<grid_e, RB_BLOCK_PRIM, RB_SMEM_CAM(RB_BLOCK_PRIM), stream>>>(scene->dev, ka, dim_base, t0, n, k1, v1);
+                void* edge_args[] = {&scene->dev, &ka, &dim_base, &t0, &n, &k1, &v1};
+                RB_CUDA_OK(cudaLaunchKernel(kern.primary_edge, grid_e, RB_BLOCK_PRIM, edge_args, RB_SMEM_CAM(RB_BLOCK_PRIM), stream));
                 launches += 2 + 4;
             }
         }

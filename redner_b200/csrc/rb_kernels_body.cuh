@@ -1,52 +1,21 @@
 // Kernels of rb_render, included by rb_kernels.cu (general instantiation, global namespace) and by rb_kernels_lean.cu
-// (feature-free instantiation, namespace rb_lean, RB_LEAN defined).  No include guard on purpose.
-#define RB_BLOCK 128
-// Threads per block of each kernel family.  The per-sample stages are walked block-synchronously (RB_PHASE_SYNC), so the block
-// size is also the number of threads that share one pass over the instruction stream; see DESIGN.md section 6 for the measurements.
-// Each kernel's block size x minimum resident blocks (the __launch_bounds__ below) is overridable with -D for A/B runs.
-// k_bwd_sweep is bound by the instruction cache (its SASS is far larger than the cache), so wide blocks that share one pass over
-// the instruction stream win; k_bwd_trace and k_bwd_sec_* stay at <= 80 registers so that more warps hide the dependent BVH and
-// edge-tree fetches.
-#ifndef RB_BLOCK_FWD
-#define RB_BLOCK_FWD 256
-#undef RB_MIN_BLOCKS_FWD
-#define RB_MIN_BLOCKS_FWD 3
-#endif
-#ifndef RB_BLOCK_TRACE
-#define RB_BLOCK_TRACE 256
-#undef RB_MIN_BLOCKS_TRACE
-#define RB_MIN_BLOCKS_TRACE 3
-#endif
-#ifndef RB_BLOCK_SEC
-#define RB_BLOCK_SEC RB_BLOCK
-#endif
-#ifndef RB_BLOCK_SWEEP
-#define RB_BLOCK_SWEEP 512
-#undef RB_MIN_BLOCKS_SWEEP
-#define RB_MIN_BLOCKS_SWEEP 1
-#endif
-#ifndef RB_BLOCK_PRIM
-#define RB_BLOCK_PRIM RB_BLOCK
-#endif
+// (feature-free instantiation, namespace rb_lean, RB_LEAN defined).  No include guard on purpose.  Both translation units
+// include rb_kernel_set.h at global scope first.
+// Threads per block and minimum resident blocks per SM (the __launch_bounds__ below) of each kernel family.  The per-sample stages
+// are walked block-synchronously (RB_PHASE_SYNC), so the block size is also the number of threads that share one pass over the
+// instruction stream; see DESIGN.md sections 2 and 6.  k_bwd_sweep is bound by the instruction cache (its SASS is far larger than
+// the cache), so wide blocks that share one pass over the instruction stream win; k_bwd_trace and k_bwd_sec_* stay at <= 80
+// registers so that more warps hide the dependent BVH and edge-tree fetches.
+constexpr int RB_BLOCK = 128;                                // k_forward_channels (2 blocks / SM)
+constexpr int RB_BLOCK_FWD = 256, RB_MIN_BLOCKS_FWD = 3;     // k_forward
+constexpr int RB_BLOCK_TRACE = 256, RB_MIN_BLOCKS_TRACE = 3; // k_bwd_trace
+constexpr int RB_BLOCK_SEC = 128, RB_MIN_BLOCKS_SEC = 6;     // k_bwd_sec_pick, k_bwd_sec_shade: 24 warps / SM at <= 80 registers
+constexpr int RB_BLOCK_SWEEP = 512, RB_MIN_BLOCKS_SWEEP = 1; // k_bwd_sweep
+constexpr int RB_BLOCK_PRIM = 128, RB_MIN_BLOCKS_PRIM = 5;   // k_primary_edge
 // dynamic shared memory: per-thread columns of the camera accumulators (k_bwd_sweep, k_primary_edge)
 #define RB_SMEM_CAM(block) ((size_t)RB_CAM_ACC * (block) * sizeof(float))
-#ifndef RB_MIN_BLOCKS_FWD
-#define RB_MIN_BLOCKS_FWD 4
-#endif
-#ifndef RB_MIN_BLOCKS_TRACE
-#define RB_MIN_BLOCKS_TRACE 4
-#endif
-#ifndef RB_MIN_BLOCKS_SEC
-#define RB_MIN_BLOCKS_SEC 6 // the edge-tree walks wait on dependent node loads: 24 warps / SM at <= 80 registers rather than 16 at 128
-#endif
-#ifndef RB_MIN_BLOCKS_SWEEP
-#define RB_MIN_BLOCKS_SWEEP 4
-#endif
 #ifndef RB_BAND_BYTES
 #define RB_BAND_BYTES (1ULL << 30) // scratch budget of one backward band (records + lists)
-#endif
-#ifndef RB_MIN_BLOCKS_BWD
-#define RB_MIN_BLOCKS_BWD 5 // k_primary_edge
 #endif
 
 // j-th owned row -> viewport row, for the round-robin stripe partition
@@ -363,7 +332,7 @@ RB_D int sec_entry(const KernelArgs& ka, const SecRange& r, long long t) {
 __global__ void __launch_bounds__(RB_BLOCK_SEC, RB_MIN_BLOCKS_SEC) k_bwd_sec_pick(const __grid_constant__ DevScene sc, const __grid_constant__ KernelArgs ka) {
     const RenderParams& rp = ka.rp;
     const SecRange r = sec_range(ka);
-    const long long n = ka.hier_persistent ? (long long)r.pad : (long long)r.total; // (the hierarchy range has its own kernel)
+    const long long n = r.total;
     RB_BLOCK_LOOP(t, n) {
         RB_PHASE_SYNC();
         if (t < n) {
@@ -386,86 +355,6 @@ __global__ void __launch_bounds__(RB_BLOCK_SEC, RB_MIN_BLOCKS_SEC) k_bwd_sec_pic
                 if ((int)(threadIdx.x & 31) == __ffs(peers) - 1) atomicAdd(&ka.edge_hist[key], (unsigned)__popc(peers));
             }
         }
-    }
-}
-// Stage 2a': the HIERARCHY part of the vertex list with persistent warps.  The 16 stochastic descents of a vertex visit between
-// ~20 and ~300 tree nodes, so in a plain "one vertex per lane" loop a warp waits for its longest walk.  Here every lane owns a resumable walk (hier_begin / hier_step / hier_end,
-// rb_secondary.cuh); a warp advances all live walks a few steps at a time and, as soon as RB_REFILL_MIN lanes have ended theirs (or
-// nobody walks), finishes those picks together and refills the lanes from a global work counter.
-// Slower than the plain kernel (rb_kernels.cu, RB_PERSISTENT_PICK): kept as an opt-in experiment.
-#ifndef RB_REFILL_MIN
-#define RB_REFILL_MIN 12
-#endif
-#ifndef RB_WALK_BURST
-#define RB_WALK_BURST 4
-#endif
-__global__ void __launch_bounds__(RB_BLOCK_SEC, RB_MIN_BLOCKS_SEC) k_bwd_sec_pick_hier(const __grid_constant__ DevScene sc, const __grid_constant__ KernelArgs ka) {
-    const RenderParams& rp = ka.rp;
-    const SecRange r = sec_range(ka);
-    const unsigned n_h = r.total - r.pad; // hierarchy slots are [pad, total)
-    unsigned* cursor = &ka.counters->hier_cursor;
-    const int lane = threadIdx.x & 31;
-    PickSetup ps;
-    HierWalk w;
-    w.sp = 0;
-    unsigned slot = 0;
-    int phase = 0; // 0 idle, 1 walking, 2 walk ended (pick to be finished), 3 no work left
-    bool exhausted = false; // (warp-uniform)
-    while (true) {
-        const unsigned walking = __ballot_sync(0xffffffffu, phase == 1);
-        const unsigned waiting = __ballot_sync(0xffffffffu, phase == 0 || phase == 2);
-        if (waiting && (__popc(waiting) >= RB_REFILL_MIN || walking == 0)) {
-            if (phase == 2) { // finish the pick of this lane's vertex
-                Real ew = 0;
-                int edge = hier_end(ps.c, w, ps.resample, ew);
-                EdgePick pk;
-                unsigned key = 0xffffffffu;
-                if (pick_finish_hier(sc, ps, edge, ew, pk)) {
-                    ka.picks[slot] = pk;
-                    key = (unsigned)pk.edge_id;
-                    unsigned peers = __match_any_sync(__activemask(), key);
-                    if (lane == __ffs(peers) - 1) atomicAdd(&ka.edge_hist[key], (unsigned)__popc(peers));
-                }
-                ka.sec_keys[slot] = key;
-                phase = 0;
-            }
-            const unsigned want = __ballot_sync(0xffffffffu, phase == 0);
-            if (!exhausted && want) {
-                const int leader = __ffs(want) - 1;
-                unsigned base = 0;
-                if (lane == leader) base = atomicAdd(cursor, (unsigned)__popc(want));
-                base = __shfl_sync(0xffffffffu, base, leader);
-                exhausted = base + (unsigned)__popc(want) >= n_h;
-                if (phase == 0) {
-                    unsigned k = base + (unsigned)__popc(want & ((1u << lane) - 1u));
-                    if (k < n_h) {
-                        slot = r.pad + k;
-                        int e = ka.vert_list[(unsigned)ka.vert_cap - 1u - k];
-                        int ts = e / ka.rec_per_sample, d = e - ts * ka.rec_per_sample;
-                        SampleId id = band_sample(rp, ka.band_i0 + ts);
-                        VertexRec cur = ka.records[e];
-                        ka.sec_vals[slot] = (unsigned)e;
-                        Sampler es = bwd_edge_sampler(sc, rp, id.pixel, id.s, d, 0);
-                        if (pick_setup(sc, cur, es, ps, nullptr, nullptr) && hier_begin(ps.c, ps.edge_sel, w)) phase = w.sp > 0 ? 1 : 2;
-                        else ka.sec_keys[slot] = 0xffffffffu; // (stays idle until the next refill)
-                    } else {
-                        phase = 3;
-                    }
-                }
-            } else if (exhausted && phase == 0) {
-                phase = 3;
-            }
-        }
-        if (__ballot_sync(0xffffffffu, phase == 1) == 0) {
-            if (__ballot_sync(0xffffffffu, phase != 3) == 0) break;
-            continue;
-        }
-#pragma unroll 1
-        for (int it = 0; it < RB_WALK_BURST; it++)
-            if (phase == 1) {
-                hier_step(ps.c, w);
-                if (w.sp == 0) phase = 2;
-            }
     }
 }
 #ifndef RB_LEAN // the counting sort does not depend on scene features
@@ -579,7 +468,7 @@ __global__ void __launch_bounds__(256) k_prim_keys(const __grid_constant__ DevSc
         vals[t] = (unsigned)t;
     }
 }
-__global__ void __launch_bounds__(RB_BLOCK_PRIM, RB_MIN_BLOCKS_BWD) k_primary_edge(const __grid_constant__ DevScene sc, const __grid_constant__ KernelArgs ka, int dim_base,
+__global__ void __launch_bounds__(RB_BLOCK_PRIM, RB_MIN_BLOCKS_PRIM) k_primary_edge(const __grid_constant__ DevScene sc, const __grid_constant__ KernelArgs ka, int dim_base,
                                                                                long long t0, int n, const unsigned* keys, const unsigned* vals) {
     extern __shared__ float cam_smem[]; // [RB_CAM_ACC][blockDim.x]
     for (int k = 0; k < RB_CAM_ACC; k++) cam_smem[k * blockDim.x + threadIdx.x] = 0.f;
@@ -596,6 +485,19 @@ __global__ void __launch_bounds__(RB_BLOCK_PRIM, RB_MIN_BLOCKS_BWD) k_primary_ed
         }
     }
     block_reduce_camera(cam_smem, ka.ds.cam_accum);
+}
+
+// The kernels of this instantiation that rb_render launches through a RenderKernels table (rb_kernel_set.h).
+RenderKernels render_kernels() {
+    RenderKernels k;
+    k.forward = (const void*)k_forward;
+    k.bwd_trace = (const void*)k_bwd_trace;
+    k.bwd_sec_pick = (const void*)k_bwd_sec_pick;
+    k.bwd_sec_shade = (const void*)k_bwd_sec_shade;
+    k.bwd_sweep = (const void*)k_bwd_sweep;
+    k.prim_keys = (const void*)k_prim_keys;
+    k.primary_edge = (const void*)k_primary_edge;
+    return k;
 }
 
 #ifndef RB_LEAN

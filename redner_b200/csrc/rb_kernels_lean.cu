@@ -1,7 +1,7 @@
 // Feature-free instantiation of the render kernels: the very same source (rb_kernels_body.cuh and every per-sample header)
 // compiled with RB_LEAN, i.e. with "no environment map, pinhole camera without lens model, channels == [radiance]" as
-// compile-time facts, inside namespace rb_lean.  rb_render launches these when the scene and the options allow it; the
-// general kernels in rb_kernels.cu cover everything else.  Measured on C2: see DESIGN.md section 6.
+// compile-time facts, inside namespace rb_lean.  rb_render launches these (rb_lean::render_kernels()) when the scene and the
+// options allow it; the general kernels in rb_kernels.cu cover everything else.  Measured on C2: see DESIGN.md section 6.
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdint.h>
@@ -15,58 +15,10 @@
 #include <vector>
 
 #include "../../include/redner_b200.h"
-#include "rb_lean_api.h"
+#include "rb_kernel_set.h"
 
 #define RB_LEAN 1
 namespace rb_lean {
 #include "rb_render.cuh"
 #include "rb_kernels_body.cuh"
 } // namespace rb_lean
-
-namespace rb_lean_api {
-using rb_lean::DevScene;
-using rb_lean::KernelArgs;
-int grid(Kernel k, int device) {
-    const void* f = nullptr;
-    int block = RB_BLOCK;
-    size_t smem = 0;
-    switch (k) {
-        case K_FORWARD: f = (const void*)rb_lean::k_forward; block = RB_BLOCK_FWD; break;
-        case K_BWD_TRACE: f = (const void*)rb_lean::k_bwd_trace; block = RB_BLOCK_TRACE; break;
-        case K_BWD_SEC_PICK: f = (const void*)rb_lean::k_bwd_sec_pick; block = RB_BLOCK_SEC; break;
-        case K_BWD_SEC_SHADE: f = (const void*)rb_lean::k_bwd_sec_shade; block = RB_BLOCK_SEC; break;
-        case K_BWD_SWEEP: f = (const void*)rb_lean::k_bwd_sweep; block = RB_BLOCK_SWEEP; smem = RB_SMEM_CAM(RB_BLOCK_SWEEP); break;
-        case K_PRIM_KEYS: f = (const void*)rb_lean::k_prim_keys; block = 256; break;
-        case K_PRIMARY_EDGE: f = (const void*)rb_lean::k_primary_edge; block = RB_BLOCK_PRIM; smem = RB_SMEM_CAM(RB_BLOCK_PRIM); break;
-    }
-    int sms = 132, per_sm = 1;
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
-    if (smem > 48 * 1024) cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, f, block, smem);
-    return sms * (per_sm < 1 ? 1 : per_sm);
-}
-void forward(const void* sc, const void* ka, int grid, cudaStream_t stream) {
-    rb_lean::k_forward<<<grid, RB_BLOCK_FWD, 0, stream>>>(*(const DevScene*)sc, *(const KernelArgs*)ka);
-}
-void bwd_trace(const void* sc, const void* ka, int grid, cudaStream_t stream) {
-    rb_lean::k_bwd_trace<<<grid, RB_BLOCK_TRACE, 0, stream>>>(*(const DevScene*)sc, *(const KernelArgs*)ka);
-}
-void bwd_sec_pick(const void* sc, const void* ka, int grid, cudaStream_t stream) {
-    rb_lean::k_bwd_sec_pick<<<grid, RB_BLOCK_SEC, 0, stream>>>(*(const DevScene*)sc, *(const KernelArgs*)ka);
-}
-void bwd_sec_pick_hier(const void* sc, const void* ka, int grid, cudaStream_t stream) {
-    rb_lean::k_bwd_sec_pick_hier<<<grid, RB_BLOCK_SEC, 0, stream>>>(*(const DevScene*)sc, *(const KernelArgs*)ka);
-}
-void bwd_sec_shade(const void* sc, const void* ka, int grid, cudaStream_t stream) {
-    rb_lean::k_bwd_sec_shade<<<grid, RB_BLOCK_SEC, 0, stream>>>(*(const DevScene*)sc, *(const KernelArgs*)ka);
-}
-void bwd_sweep(const void* sc, const void* ka, int grid, cudaStream_t stream) {
-    rb_lean::k_bwd_sweep<<<grid, RB_BLOCK_SWEEP, RB_SMEM_CAM(RB_BLOCK_SWEEP), stream>>>(*(const DevScene*)sc, *(const KernelArgs*)ka);
-}
-void prim_keys(const void* sc, const void* ka, int dim_base, long long t0, int n, unsigned* keys, unsigned* vals, int grid, cudaStream_t stream) {
-    rb_lean::k_prim_keys<<<grid, 256, 0, stream>>>(*(const DevScene*)sc, *(const KernelArgs*)ka, dim_base, t0, n, keys, vals);
-}
-void primary_edge(const void* sc, const void* ka, int dim_base, long long t0, int n, const unsigned* keys, const unsigned* vals, int grid, cudaStream_t stream) {
-    rb_lean::k_primary_edge<<<grid, RB_BLOCK_PRIM, RB_SMEM_CAM(RB_BLOCK_PRIM), stream>>>(*(const DevScene*)sc, *(const KernelArgs*)ka, dim_base, t0, n, keys, vals);
-}
-} // namespace rb_lean_api

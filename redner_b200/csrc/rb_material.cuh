@@ -39,12 +39,7 @@ RB_HD Real tex_level(const rb_texture& t, V2 du, V2 dv, Real& fu, Real& fv) {
     return log2(rb_max(rb_max(fu, fv), Real(1e-8)));
 }
 // Mip-mapped (trilinear) fetch; out of line: ~15 inlined copies per kernel otherwise.  out[0..nch)
-#ifndef RB_INLINE_TEX
-#define RB_TEX_FN RB_FN
-#else
-#define RB_TEX_FN RB_HD
-#endif
-RB_TEX_FN void tex_eval_mip(const rb_texture& t, int nch, V2 uv_, V2 du_dxy_, V2 dv_dxy_, Real* out) {
+RB_FN void tex_eval_mip(const rb_texture& t, int nch, V2 uv_, V2 du_dxy_, V2 dv_dxy_, Real* out) {
     Real sx = t.uv_scale[0], sy = t.uv_scale[1];
     V2 uv = mk2(uv_.x * sx, uv_.y * sy);
     V2 du = du_dxy_ * sx, dv = dv_dxy_ * sy;

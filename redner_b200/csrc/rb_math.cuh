@@ -30,16 +30,6 @@ typedef float Real;
 #endif
 #define RB_FN inline __host__ __device__ __noinline__
 #define RB_DFN inline __device__ __noinline__
-// Rarely used features (environment map, non-pinhole cameras, lens model, G-buffer channels).  Taking them out of line costs the
-// hot kernels an ABI call that spills the caller's live state, so they are inlined like everything else unless RB_COLD_OUTLINE
-// is defined.
-#ifdef RB_COLD_OUTLINE
-#define RB_COLD RB_FN
-#define RB_COLD_D RB_DFN
-#else
-#define RB_COLD RB_HD
-#define RB_COLD_D RB_D
-#endif
 
 // Feature tests.  rb_kernels_lean.cu compiles the same kernels a second time with RB_LEAN defined: no environment map, pinhole
 // camera without lens model, channels == [radiance] -- the configuration of nearly every optimisation loop.  There the

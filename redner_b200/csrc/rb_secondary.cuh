@@ -195,9 +195,8 @@ RB_D void split_samples(int num, Real prob0, Real& u, int& n0, int& n1) {
         }
     }
 }
-// 16 correlated stochastic descents through both trees followed by reservoir resampling among the reached leaves, as three
-// resumable pieces: hier_begin, hier_step (ONE stack item per call) and hier_end.  sample_edge_hier runs them back to back; the
-// persistent kernel k_bwd_sec_pick_hier interleaves the steps of 32 vertices and refills lanes whose walk has ended.
+// 16 correlated stochastic descents through both trees followed by reservoir resampling among the reached leaves, in three
+// pieces: hier_begin, hier_step (ONE stack item per call) and hier_end.  sample_edge_hier runs them back to back.
 struct HierWalk {
     StackH stack[RB_EDGE_STACK_H];
     StackH leaves[RB_EDGE_H_SAMPLES];
@@ -221,16 +220,6 @@ RB_D bool hier_begin(const EdgeCtx& c, Real u, HierWalk& w) {
 // Interior nodes first, leaves afterwards (in the order the descent reached them, so the reservoir of hier_end consumes
 // `resample_u` exactly as a combined loop would): lanes of a warp would otherwise sit in the leaf branch (silhouette
 // test + LTC line integral) and the interior branch (two box bounds) of the same loop at the same time.
-// Record of an inner node that has just been pushed: start fetching it now -- it is popped a few dozen to a few hundred
-// instructions later and the walk is bound by exactly these dependent fetches.
-RB_D void edge_node_prefetch(const DevScene& sc, int ref) {
-#if defined(__CUDA_ARCH__) && defined(RB_EDGE_PREFETCH)
-    if (ref >= 0) asm volatile("prefetch.global.L1 [%0];" ::"l"(sc.edge_nodes + ref));
-#else
-    (void)sc;
-    (void)ref;
-#endif
-}
 RB_D void hier_step(const EdgeCtx& c, HierWalk& w) { // requires w.sp > 0
     const DevScene& sc = *c.sc;
     StackH it = w.stack[--w.sp];
@@ -254,8 +243,6 @@ RB_D void hier_step(const EdgeCtx& c, HierWalk& w) { // requires w.sp > 0
         Real p0 = i0 / (i0 + i1);
         int n0, n1;
         split_samples(it.num, p0, w.u, n0, n1);
-        if (n0 > 0) edge_node_prefetch(sc, n.c[0].ref);
-        if (n1 > 0) edge_node_prefetch(sc, n.c[1].ref);
         if (n0 > 0 && w.sp < RB_EDGE_STACK_H) { w.stack[w.sp].node = n.c[0].ref; w.stack[w.sp].num = (short)n0; w.stack[w.sp].is6d = it.is6d; w.stack[w.sp].pmf = it.pmf * p0; w.sp++; }
         if (n1 > 0 && w.sp < RB_EDGE_STACK_H) { w.stack[w.sp].node = n.c[1].ref; w.stack[w.sp].num = (short)n1; w.stack[w.sp].is6d = it.is6d; w.stack[w.sp].pmf = it.pmf * (1 - p0); w.sp++; }
     }
@@ -383,8 +370,7 @@ struct alignas(16) EdgePick {
     V3 sample_p, mwt;
 };
 // The pick in three pieces -- pick_setup (frame, lobe, LTC matrices, strategy), the edge choice (hierarchy walk or gather), and
-// pick_finish_hier (point on the chosen edge by inverting the LTC line CDF) -- so that the persistent hierarchy kernel can interleave
-// the walks of many vertices; secondary_edge_pick runs them back to back.
+// pick_finish_hier (point on the chosen edge by inverting the LTC line CDF); secondary_edge_pick runs them back to back.
 struct PickSetup {
     EdgeCtx c;
     Real m_pmf, nee_pmf, edge_sel, resample, t_sel;
