@@ -18,18 +18,6 @@ constexpr int RB_BLOCK_PRIM = 128, RB_MIN_BLOCKS_PRIM = 5;   // k_primary_edge
 #define RB_BAND_BYTES (1ULL << 30) // scratch budget of one backward band (records + lists)
 #endif
 
-// j-th owned row -> viewport row, for the round-robin stripe partition
-RB_D int owned_row_to_row(const RenderParams& rp, int j) {
-    int s = j / rp.rows_per_stripe, w = j % rp.rows_per_stripe;
-    return (s * rp.num_parts + rp.part) * rp.rows_per_stripe + w;
-}
-static int count_owned_rows(int H, int part, int num_parts, int rps) {
-    int n = 0;
-    for (int r = 0; r < H; r++)
-        if ((r / rps) % num_parts == part) n++;
-    return n;
-}
-
 struct WorkItem {
     bool valid;
     int pixel;    // viewport-relative pixel id (y * vp_w + x)
@@ -165,23 +153,7 @@ __global__ void __launch_bounds__(RB_BLOCK, 2) k_forward_channels(const __grid_c
             int o0 = __shfl_xor_sync(0xffffffffu, ids[0], off), o1 = __shfl_xor_sync(0xffffffffu, ids[1], off), o2 = __shfl_xor_sync(0xffffffffu, ids[2], off);
             if (ol > last) { last = ol; ids[0] = o0; ids[1] = o1; ids[2] = o2; }
         }
-        if (w.valid && w.sample_lane == 0) {
-            float* px = ka.image + (size_t)rp.nd * w.pixel;
-            int d = 0;
-            for (int c = 0; c < rp.num_channels; c++) {
-                int ch = rp.channels[c];
-                int width = (ch == RB_CH_RADIANCE || ch == RB_CH_POSITION || ch == RB_CH_GEOMETRY_NORMAL || ch == RB_CH_SHADING_NORMAL ||
-                             ch == RB_CH_DIFFUSE_REFLECTANCE || ch == RB_CH_SPECULAR_REFLECTANCE || ch == RB_CH_VERTEX_COLOR) ? 3
-                          : (ch == RB_CH_UV || ch == RB_CH_BARYCENTRIC) ? 2 : (ch == RB_CH_GENERIC_TEXTURE ? rp.max_generic : 1);
-                if (ch == RB_CH_SHAPE_ID || ch == RB_CH_TRIANGLE_ID || ch == RB_CH_MATERIAL_ID) {
-                    int v = ids[ch - RB_CH_SHAPE_ID];
-                    if (last >= 0 && d < nd) px[d] = (float)v;
-                } else {
-                    for (int i = 0; i < width && d + i < nd; i++) px[d + i] += acc[d + i];
-                }
-                d += width;
-            }
-        }
+        if (w.valid && w.sample_lane == 0) write_gbuffer_pixel(rp, acc, ids, last >= 0, ka.image + (size_t)rp.nd * w.pixel);
     }
 }
 

@@ -1,5 +1,5 @@
-// Per-sample render logic, shared by the CUDA kernels (rb_kernels.cu) and by the host-compiled debug emulator
-// (tools/cpu_emu, development aid only).  One call == one (pixel, sample) or one primary-edge sample.
+// Per-sample render logic and the render set-up, shared by the CUDA kernels and their driver (rb_kernels.cu) and by the
+// host-compiled debug emulator (tools/cpu_emu, development aid only).  One call == one (pixel, sample) or one primary-edge sample.
 //   forward_sample         src/pathtracer.cpp:240-390 for one pixel-sample
 //   backward_sample        src/pathtracer.cpp:392-762 (reverse sweep, first-hit adjoint)
 //   primary_edge_sample    src/edge.cpp:385-625 + src/pathtracer.cpp:766-942 + src/edge.cpp:700-783
@@ -9,7 +9,8 @@
 #include "rb_path.cuh"
 #include "rb_secondary.cuh"
 
-#define RB_MAX_SWEEP_DEPTH 64 // emulator-only bound of the fused composition
+#define RB_MAX_ND 64                // floats per pixel of an image, at most
+#define RB_MAX_BOUNDARY_BOUNCES 64  // bounces the boundary stage supports: one bit per depth in KernelArgs::vmask
 // Phase barrier: the warps of a block enter each stage of a sample together, so one instruction-cache miss serves the
 // whole block (measured 2.1x - 7.4x on the backward pass, DESIGN.md "instruction supply").  Every call site is reached
 // by all threads of the block: the kernels iterate block-uniformly and pass an `act` flag instead of branching around.
@@ -57,6 +58,110 @@ RB_HD int rb_channel_width(int ch, int max_generic) { // floats of one channel, 
         default: return 1;
     }
 }
+
+// Row partition over devices: round-robin stripes of `rows_per_stripe` viewport rows, stripe k rendered by part k % num_parts.
+// j-th owned row -> viewport row
+RB_HD int owned_row_to_row(const RenderParams& rp, int j) {
+    int s = j / rp.rows_per_stripe, w = j % rp.rows_per_stripe;
+    return (s * rp.num_parts + rp.part) * rp.rows_per_stripe + w;
+}
+inline int count_owned_rows(int H, int part, int num_parts, int rps) {
+    int n = 0;
+    for (int r = 0; r < H; r++)
+        if ((r / rps) % num_parts == part) n++;
+    return n;
+}
+
+// ---- render set-up shared by both rb_render drivers: the kernels' (rb_kernels.cu) and the host emulator's (tools/cpu_emu)
+// Fills `ka` from the options, the scene's camera, generic-texture width and partition, and the image pointers.  Returns the
+// error message, or null.  An empty viewport or zero samples passes: there is nothing to render then.
+inline const char* setup_kernel_args(const rb_options& opt, const rb_camera& cam, int max_generic, int part, int num_parts, int rows_per_stripe,
+                                     float* image, const float* d_image, const rb_dscene_desc* d_scene, float* screen_grad, KernelArgs& ka) {
+    if (image == nullptr && d_image == nullptr) return "rb_render: neither rendered_image nor d_rendered_image given";
+    if (d_image != nullptr && d_scene == nullptr) return "rb_render: d_rendered_image given without d_scene";
+    if (opt.max_bounces < 0 || opt.num_samples < 0) return "rb_render: negative max_bounces / num_samples";
+    memset(&ka, 0, sizeof(ka));
+    RenderParams& rp = ka.rp;
+    rp.seed = opt.seed;
+    rp.spp = opt.num_samples;
+    rp.max_bounces = opt.max_bounces;
+    rp.sampler_type = opt.sampler_type;
+    rp.sample_pixel_center = opt.sample_pixel_center;
+    rp.num_channels = opt.num_channels;
+    rp.max_generic = max_generic;
+    rp.rad_dim = -1;
+    if (opt.num_channels > RB_CH_COUNT) return "rb_render: too many channels";
+    for (int i = 0; i < opt.num_channels; i++) {
+        rp.channels[i] = opt.channels[i];
+        if (opt.channels[i] < 0 || opt.channels[i] >= RB_CH_COUNT) return "rb_render: unknown channel";
+        if (opt.channels[i] == RB_CH_RADIANCE) {
+            if (rp.rad_dim != -1) return "Duplicated radiance channel"; // src/channels.cpp:24-26
+            // the reference stores the CHANNEL INDEX and uses it as a float offset (src/channels.cpp:27,
+            // src/path_contribution.cpp:125-129); identical whenever radiance is the first channel
+            rp.rad_dim = i;
+        }
+    }
+    rp.only_radiance = opt.num_channels == 1 && opt.channels[0] == RB_CH_RADIANCE ? 1 : 0;
+    rp.nd = 0;
+    rp.rad_off = -1;
+    for (int i = 0; i < opt.num_channels; i++) {
+        if (opt.channels[i] == RB_CH_RADIANCE) rp.rad_off = rp.nd;
+        rp.nd += rb_channel_width(opt.channels[i], max_generic);
+    }
+    if (rp.nd > RB_MAX_ND) return "rb_render: more than 64 image dimensions requested";
+    rp.part = part;
+    rp.num_parts = num_parts;
+    rp.rows_per_stripe = rows_per_stripe;
+    rp.vp_w = cam.viewport_end[0] - cam.viewport_beg[0];
+    rp.vp_h = cam.viewport_end[1] - cam.viewport_beg[1];
+    int L = 1;
+    while (L * 2 <= 32 && L * 2 <= rp.spp) L *= 2;
+    ka.lanes_per_pixel = L;
+    ka.owned_rows = count_owned_rows(rp.vp_h, part, num_parts, rows_per_stripe);
+    ka.image = image;
+    ka.d_image = d_image;
+    ka.screen_grad = screen_grad;
+    return nullptr;
+}
+// The boundary (secondary-edge) stage of the backward pass runs: it needs edges, a light and a radiance channel.
+RB_HD bool boundary_stage_runs(const DevScene& sc, const RenderParams& rp) {
+    return sc.use_secondary_edge && sc.num_edges > 0 && sc.num_lights > 0 && rp.rad_dim >= 0;
+}
+// The primary-edge pass of the backward pass runs.
+RB_HD bool primary_edge_pass_runs(const DevScene& sc) { return sc.use_primary_edge && sc.num_edges > 0 && sc.prim_edge_cdf != nullptr; }
+// Checks the gradient descriptor against the scene and the options, and points the environment-map gradients of `ka.ds` at
+// d_scene's.  Returns the error message, or null.  Each driver fills the shape, material, light and camera gradients itself.
+inline const char* setup_backward(const rb_dscene_desc& d_scene, const DevScene& sc, KernelArgs& ka) {
+    if (d_scene.num_shapes != sc.num_shapes || d_scene.num_materials != sc.num_materials || d_scene.num_lights != sc.num_lights - (sc.has_envmap ? 1 : 0))
+        return "rb_render: d_scene does not match the scene (shape / material / light counts)";
+    if (boundary_stage_runs(sc, ka.rp) && ka.rp.max_bounces > RB_MAX_BOUNDARY_BOUNCES) return "rb_render: secondary edge sampling supports at most 64 bounces";
+    memset(&ka.ds.env_values, 0, sizeof(rb_texture));
+    ka.ds.env_w2e = nullptr;
+    if (d_scene.envmap != nullptr) {
+        ka.ds.env_values = d_scene.envmap->values;
+        ka.ds.env_w2e = d_scene.envmap->world_to_env;
+    } else if (sc.has_envmap) {
+        return "rb_render: the scene has an environment map but d_scene has no envmap gradient buffers";
+    }
+    return nullptr;
+}
+// Writes one G-buffer pixel from the sums over its samples (`acc`) and the ids of the last sample that hit (`hit`: some sample
+// did): channel sums are added to the pixel, id channels are overwritten.
+RB_HD void write_gbuffer_pixel(const RenderParams& rp, const float* acc, const int* ids, bool hit, float* px) {
+    const int nd = rp.nd < RB_MAX_ND ? rp.nd : RB_MAX_ND;
+    int d = 0;
+    for (int c = 0; c < rp.num_channels; c++) {
+        int ch = rp.channels[c];
+        int width = rb_channel_width(ch, rp.max_generic);
+        if (ch == RB_CH_SHAPE_ID || ch == RB_CH_TRIANGLE_ID || ch == RB_CH_MATERIAL_ID) {
+            if (hit && d < nd) px[d] = (float)ids[ch - RB_CH_SHAPE_ID];
+        } else {
+            for (int i = 0; i < width && d + i < nd; i++) px[d + i] += acc[d + i];
+        }
+        d += width;
+    }
+}
+
 RB_HD unsigned long long main_draws_per_sample(const RenderParams& rp) {
     return (unsigned long long)((rp.sample_pixel_center ? 0 : 2) + 7 * rp.max_bounces);
 }
@@ -69,6 +174,7 @@ RB_HD int secondary_edge_dim_base(const RenderParams& rp, int depth) {
     for (int d = rp.max_bounces - 1; d > depth; d--) off += 4 + 7 * (rp.max_bounces - 1 - d);
     return off;
 }
+// (not boundary_stage_runs: the reference reserves these dimensions whenever secondary edge sampling is on and a light exists)
 RB_HD int primary_edge_dim_base(const DevScene& sc, const RenderParams& rp) {
     return (sc.use_secondary_edge && sc.num_lights > 0) ? secondary_edge_dim_base(rp, -1) : 0;
 }
@@ -121,7 +227,6 @@ RB_D V3 forward_sample(const DevScene& sc, const RenderParams& rp, int pixel, in
 
 // Values of every non-radiance, non-id channel at a first hit, at their float offsets in vals[0..nd) (unweighted;
 // src/primary_contribution.cpp:36-253).  Radiance and id slots are left untouched.
-#define RB_MAX_ND 64
 RB_D void channel_values_at_hit(const DevScene& sc, const RenderParams& rp, const Isect& is, const SurfacePoint& sp, const Ray& ray, Real* vals) {
     const rb_shape& shape = sc.shapes[is.shape_id];
     const rb_material& mat = sc.materials[shape.material_id];
@@ -435,11 +540,9 @@ RB_D int backward_sample(const DevScene& sc, const KernelArgs& ka, int pixel, in
     const RenderParams& rp = ka.rp;
     int nrec = bwd_trace(sc, rp, pixel, px, py, s, recs, 1);
     if (nrec < 0) return -1;
-    V3 dpos[RB_MAX_SWEEP_DEPTH];
-    bool sec = sc.use_secondary_edge && sc.num_edges > 0 && rp.rad_dim >= 0;
-    for (int d = 0; d < nrec && d < RB_MAX_SWEEP_DEPTH; d++) {
-        dpos[d] = sec ? bwd_secondary(sc, ka, pixel, s, d, recs[d]) : zero3();
-    }
+    V3 dpos[RB_MAX_BOUNDARY_BOUNCES]; // (setup_backward rejects deeper paths when the stage runs)
+    const bool sec = boundary_stage_runs(sc, rp);
+    for (int d = 0; sec && d < nrec; d++) dpos[d] = bwd_secondary(sc, ka, pixel, s, d, recs[d]);
     bwd_sweep(sc, ka, pixel, px, py, s, recs, 1, nrec, sec ? dpos : nullptr, cam_acc);
     return nrec;
 }

@@ -303,9 +303,8 @@ static int fetch_mesh(const rb_shape& s, HostMesh& m, cudaStream_t stream) {
     return 0;
 }
 
-static std::vector<HostMesh>& host_meshes(rb_scene* sc) {
+static std::vector<HostMesh>& host_meshes() {
     static thread_local std::vector<HostMesh> meshes;
-    (void)sc;
     return meshes;
 }
 
@@ -317,7 +316,7 @@ int rb_build_lights(rb_scene* sc, cudaStream_t stream) {
     if (sc->dev.num_lights == 0) return 0;
     HostLightTables t;
     std::string err;
-    if (!host_build_lights(sc->lights, host_meshes(sc), t, err, env, env ? sc->dev.env.pdf_norm : 0.0, env ? host_bsphere_radius(host_meshes(sc)) : 0.0)) {
+    if (!host_build_lights(sc->lights, host_meshes(), t, err, env, env ? sc->dev.env.pdf_norm : 0.0, env ? host_bsphere_radius(host_meshes()) : 0.0)) {
         rb_set_error(err);
         return 1;
     }
@@ -365,10 +364,10 @@ int rb_build_edges(rb_scene* sc, cudaStream_t stream) {
         return 0;
     }
     HostEdgeTables t;
-    host_build_edges(sc->shapes, host_meshes(sc), sc->dev.cam, false, t);
+    host_build_edges(sc->shapes, host_meshes(), sc->dev.cam, false, t);
     int E = (int)t.edges.size();
     const bool host_tables = getenv("RB_HOST_TREES") != nullptr || (E < RB_GPU_TABLES_MIN_EDGES && getenv("RB_GPU_TREES") == nullptr);
-    if (host_tables && sc->dev.use_primary_edge != 0) host_primary_edge_distribution(sc->shapes, host_meshes(sc), sc->dev.cam, t);
+    if (host_tables && sc->dev.use_primary_edge != 0) host_primary_edge_distribution(sc->shapes, host_meshes(), sc->dev.cam, t);
     sc->dev.num_edges = E;
     if (E == 0) return 0;
     Edge* d_edges;
@@ -389,7 +388,7 @@ int rb_build_edges(rb_scene* sc, cudaStream_t stream) {
             if (rb_build_edge_trees_gpu(sc, stream)) return 1;
         } else {
             HostEdgeTree tree;
-            host_build_edge_tree(sc->shapes, host_meshes(sc), t.edges, sc->dev.cam, tree);
+            host_build_edge_tree(sc->shapes, host_meshes(), t.edges, sc->dev.cam, tree);
             EdgeNode* d_nodes;
             sc->num_edge_nodes = (int)tree.nodes.size();
             if (tree.nodes.empty()) tree.nodes.push_back(EdgeNode()); // (single-edge trees have no inner node)
@@ -484,32 +483,12 @@ extern "C" int rb_scene_create_on_stream(const rb_scene_desc* desc, rb_scene** o
 
     sc->shapes.assign(desc->shapes, desc->shapes + desc->num_shapes);
     sc->materials.assign(desc->materials, desc->materials + desc->num_materials);
-    for (int l = 0; l < desc->num_lights; l++) {
-        DevLight dl;
-        dl.shape_id = desc->lights[l].shape_id;
-        for (int k = 0; k < 3; k++) dl.intensity[k] = desc->lights[l].intensity[k];
-        dl.two_sided = desc->lights[l].two_sided;
-        dl.directly_visible = desc->lights[l].directly_visible;
-        if (dl.shape_id < 0 || dl.shape_id >= desc->num_shapes) {
-            rb_set_error("rb_scene_create: area light refers to an invalid shape");
-            return fail();
-        }
-        sc->lights.push_back(dl);
+    if (const char* err = host_check_scene_desc(*desc)) {
+        rb_set_error(err);
+        return fail();
     }
-    for (int s = 0; s < desc->num_shapes; s++) {
-        const rb_shape& sh = sc->shapes[s];
-        if (sh.material_id < 0 || sh.material_id >= desc->num_materials) {
-            rb_set_error("rb_scene_create: shape refers to an invalid material");
-            return fail();
-        }
-        if (sh.vertices == nullptr || sh.indices == nullptr) {
-            rb_set_error("rb_scene_create: shape without vertices / indices");
-            return fail();
-        }
-    }
-    sc->max_generic_texture_dimension = 0;
-    for (const rb_material& m : sc->materials)
-        if (m.generic_texture.num_levels > 0) sc->max_generic_texture_dimension = std::max(sc->max_generic_texture_dimension, m.generic_texture.channels);
+    sc->lights = host_area_lights(*desc);
+    sc->max_generic_texture_dimension = host_max_generic_texture_dimension(*desc);
 
     rb_shape* d_shapes;
     rb_material* d_materials;
@@ -540,7 +519,7 @@ extern "C" int rb_scene_create_on_stream(const rb_scene_desc* desc, rb_scene** o
     for (const rb_shape& s : sc->shapes) num_triangles += s.num_triangles;
     sc->edge_list_on_device = need_edges && getenv("RB_HOST_TREES") == nullptr && getenv("RB_HOST_EDGE_LIST") == nullptr &&
                               (num_triangles >= RB_GPU_EDGE_LIST_MIN_TRIANGLES || getenv("RB_GPU_TREES") != nullptr || getenv("RB_GPU_EDGE_LIST") != nullptr);
-    auto& meshes = host_meshes(sc);
+    auto& meshes = host_meshes();
     meshes.assign(sc->shapes.size(), HostMesh());
     std::vector<char> need(sc->shapes.size(), ((need_edges && !sc->edge_list_on_device) || desc->envmap != nullptr) ? 1 : 0); // (envmap: bounding sphere of everything)
     for (const DevLight& l : sc->lights) need[l.shape_id] = 1;
@@ -550,17 +529,7 @@ extern "C" int rb_scene_create_on_stream(const rb_scene_desc* desc, rb_scene** o
         rb_set_error("rb_scene_create: device-to-host geometry copy failed (are the shape buffers device pointers?)");
         return fail();
     }
-    sc->dev.has_envmap = desc->envmap != nullptr;
-    if (sc->dev.has_envmap) {
-        const rb_envmap& e = *desc->envmap;
-        sc->dev.env.values = e.values;
-        memcpy(sc->dev.env.w2e, e.world_to_env, sizeof(sc->dev.env.w2e));
-        memcpy(sc->dev.env.e2w, e.env_to_world, sizeof(sc->dev.env.e2w));
-        sc->dev.env.cdf_ys = e.sample_cdf_ys;
-        sc->dev.env.cdf_xs = e.sample_cdf_xs;
-        sc->dev.env.pdf_norm = e.pdf_norm;
-        sc->dev.env.directly_visible = e.directly_visible;
-    }
+    host_setup_envmap(desc->envmap, sc->dev);
     if (rb_build_lights(sc, stream)) return fail();
     auto t2 = std::chrono::high_resolution_clock::now();
     if (rb_build_edges(sc, stream)) return fail();
@@ -626,9 +595,6 @@ extern "C" int rb_scene_set_camera(rb_scene* sc, const rb_camera* cam) {
     if (cam->width <= 0 || cam->height <= 0 || cam->viewport_end[0] <= cam->viewport_beg[0] || cam->viewport_end[1] <= cam->viewport_beg[1]) {
         rb_set_error("rb_scene_set_camera: empty image / viewport");
         return 1;
-    }
-    if ((cam->camera_type != RB_CAMERA_PERSPECTIVE || cam->has_distortion) && sc->dev.cam.type == RB_CAMERA_PERSPECTIVE && !sc->dev.cam.has_distortion) {
-        // (allowed; the general kernels serve it)
     }
     int prev = 0;
     cudaGetDevice(&prev);

@@ -28,6 +28,49 @@ struct HostEdgeTables {
     std::vector<double> prim_pmf, prim_cdf;
 };
 
+// ---- scene descriptor -> scene, shared by both rb_scene_create (rb_scene.cu and the emulator's)
+// Index checks of the descriptor; returns the error message, or null.
+inline const char* host_check_scene_desc(const rb_scene_desc& desc) {
+    for (int l = 0; l < desc.num_lights; l++)
+        if (desc.lights[l].shape_id < 0 || desc.lights[l].shape_id >= desc.num_shapes) return "rb_scene_create: area light refers to an invalid shape";
+    for (int s = 0; s < desc.num_shapes; s++) {
+        const rb_shape& sh = desc.shapes[s];
+        if (sh.material_id < 0 || sh.material_id >= desc.num_materials) return "rb_scene_create: shape refers to an invalid material";
+        if (sh.vertices == nullptr || sh.indices == nullptr) return "rb_scene_create: shape without vertices / indices";
+    }
+    return nullptr;
+}
+inline std::vector<DevLight> host_area_lights(const rb_scene_desc& desc) {
+    std::vector<DevLight> out;
+    for (int l = 0; l < desc.num_lights; l++) {
+        DevLight dl;
+        dl.shape_id = desc.lights[l].shape_id;
+        for (int k = 0; k < 3; k++) dl.intensity[k] = desc.lights[l].intensity[k];
+        dl.two_sided = desc.lights[l].two_sided;
+        dl.directly_visible = desc.lights[l].directly_visible;
+        out.push_back(dl);
+    }
+    return out;
+}
+inline int host_max_generic_texture_dimension(const rb_scene_desc& desc) {
+    int n = 0;
+    for (int m = 0; m < desc.num_materials; m++)
+        if (desc.materials[m].generic_texture.num_levels > 0) n = std::max(n, desc.materials[m].generic_texture.channels);
+    return n;
+}
+// The environment map of the descriptor (may be null) -> has_envmap and env of the scene.
+inline void host_setup_envmap(const rb_envmap* e, DevScene& d) {
+    d.has_envmap = e != nullptr;
+    if (!e) return;
+    d.env.values = e->values;
+    memcpy(d.env.w2e, e->world_to_env, sizeof(d.env.w2e));
+    memcpy(d.env.e2w, e->env_to_world, sizeof(d.env.e2w));
+    d.env.cdf_ys = e->sample_cdf_ys;
+    d.env.cdf_xs = e->sample_cdf_xs;
+    d.env.pdf_norm = e->pdf_norm;
+    d.env.directly_visible = e->directly_visible;
+}
+
 // Radius of the scene's bounding sphere as the reference computes it (src/scene.cpp:156-195) -- including its slip of
 // folding each shape's Y extent into the Z bounds; the radius only scales the environment map's selection weight.
 inline double host_bsphere_radius(const std::vector<HostMesh>& meshes) {

@@ -44,7 +44,7 @@ def all_reduce_packed(tensors: Sequence[torch.Tensor], group=None) -> List[torch
 
 
 def owned_rows(height: int, rank: int, world: int, rows_per_stripe: int = 4) -> List[int]:
-    """Rows of the viewport rendered by `rank` (mirrors count_owned_rows / owned_row_to_row in rb_kernels.cu)."""
+    """Rows of the viewport rendered by `rank` (mirrors count_owned_rows / owned_row_to_row in csrc/rb_render.cuh)."""
     return [r for r in range(height) if (r // rows_per_stripe) % world == rank]
 
 

@@ -50,6 +50,40 @@ def check_batch_of_views(rb, dev):
             assert pu.rel_l2(g_batch[key].numpy(), g_single[key].numpy()) < 1e-5, key
 
 
+def check_rejected_options(rb, dev):
+    """rb_render rejects a duplicated radiance channel, an unknown channel, more than 64 image dimensions and more than 64 bounces with
+    secondary edge sampling, with the library's messages.  Called through the C ABI: the Python shim refuses an unknown channel itself."""
+    import ctypes as C
+    import scenes
+    from redner_b200 import _lib as L, api
+    sc = scenes.corner_ball(dev, resolution=(8, 8), variant="generic")  # (a 5-channel generic texture; differentiable, so edges are sampled)
+    args = api.RenderFunction.serialize_scene(sc, 1, 1, sampler_type=rb.SamplerType.sobol, device=dev, backend=rb,
+                                              use_primary_edge_sampling=True, use_secondary_edge_sampling=True)
+    scene = api.RenderFunction._unpack((1, 2), args).scene
+    lib = L._lib
+    image = (C.c_float * (8 * 8 * 128))()
+    d_image = (C.c_float * (8 * 8 * 3))()
+    light_grads = [(C.c_float * 3)() for _ in range(2)]
+    d_shapes, d_mats = (L.rb_dshape * 4)(), (L.rb_material * 3)()
+    d_lights = (C.c_void_p * 2)(*[C.addressof(g) for g in light_grads])
+    d_scene = L.rb_dscene_desc(num_shapes=4, shapes=d_shapes, num_materials=3, materials=d_mats, num_lights=2, light_intensity=d_lights)
+
+    def render(channels, max_bounces=1, backward=False):
+        o = L.rb_options(seed=1, num_samples=1, max_bounces=max_bounces, num_channels=len(channels), sampler_type=1, sample_pixel_center=0)
+        chs = (C.c_int * len(channels))(*channels)
+        o.channels = chs
+        rc = lib.rb_render(scene._handle, C.byref(o), None if backward else image, d_image if backward else None, C.byref(d_scene) if backward else None,
+                           None, None)
+        return rc, L.last_error(lib)
+
+    radiance, generic = int(rb.channels.radiance), int(rb.channels.generic_texture)
+    assert render([radiance]) == (0, "")
+    assert render([radiance, radiance]) == (1, "Duplicated radiance channel")
+    assert render([radiance, 99]) == (1, "rb_render: unknown channel")
+    assert render([generic] * 13) == (1, "rb_render: more than 64 image dimensions requested")
+    assert render([radiance], max_bounces=65, backward=True) == (1, "rb_render: secondary edge sampling supports at most 64 bounces")
+
+
 def main():
     so, names = sys.argv[1], sys.argv[2:]
     import torch
@@ -58,9 +92,10 @@ def main():
     from redner_b200 import redner as rb
     import parity_utils as pu
     dev = torch.device("cpu")
+    checks = {"batch_of_views": check_batch_of_views, "rejected_options": check_rejected_options}
     for name in names:
-        if name == "batch_of_views":
-            check_batch_of_views(rb, dev)
+        if name in checks:
+            checks[name](rb, dev)
             print("ok", name, flush=True)
             continue
         if name in pu.STAT_CASES:

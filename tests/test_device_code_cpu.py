@@ -83,6 +83,13 @@ def test_batch_of_views_through_one_native_scene(emulator):
     _check(emulator, ["batch_of_views"])
 
 
+def test_render_options_are_rejected_like_the_library(emulator):
+    """The emulator's rb_render makes the library's decisions (the render set-up in rb_render.cuh is shared): a duplicated radiance
+    channel, an unknown channel, more than 64 image dimensions and more than 64 bounces with secondary edges are each refused with
+    the library's message."""
+    _check(emulator, ["rejected_options"])
+
+
 def test_lean_instantiation_meets_the_goldens_it_serves(emulator_lean):
     names = [n for n, c in pu.CASES.items() if "channels" not in c and c["scene"] in ("single_triangle", "shadow_blocker", "glossy_room", "nmap_room")]
     assert len(names) >= 7

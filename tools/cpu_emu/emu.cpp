@@ -72,22 +72,18 @@ static int build_node(rb_scene* sc, std::vector<int>& order, std::vector<float>&
 }
 
 extern "C" int rb_scene_create(const rb_scene_desc* desc, rb_scene** out) {
+    if (const char* err = host_check_scene_desc(*desc)) {
+        g_err = err;
+        return 1;
+    }
     rb_scene* sc = new rb_scene();
     memset(&sc->dev, 0, sizeof(DevScene));
     sc->cam = desc->camera;
     host_setup_camera(desc->camera, sc->dev.cam);
     sc->shapes.assign(desc->shapes, desc->shapes + desc->num_shapes);
     sc->materials.assign(desc->materials, desc->materials + desc->num_materials);
-    for (int l = 0; l < desc->num_lights; l++) {
-        DevLight dl;
-        dl.shape_id = desc->lights[l].shape_id;
-        for (int k = 0; k < 3; k++) dl.intensity[k] = desc->lights[l].intensity[k];
-        dl.two_sided = desc->lights[l].two_sided;
-        dl.directly_visible = desc->lights[l].directly_visible;
-        sc->lights.push_back(dl);
-    }
-    for (const rb_material& m : sc->materials)
-        if (m.generic_texture.num_levels > 0) sc->max_generic = std::max(sc->max_generic, m.generic_texture.channels);
+    sc->lights = host_area_lights(*desc);
+    sc->max_generic = host_max_generic_texture_dimension(*desc);
     DevScene& d = sc->dev;
     d.edge_root_cs = d.edge_root_ncs = RB_EDGE_EMPTY;
     d.shapes = sc->shapes.data();
@@ -144,19 +140,8 @@ extern "C" int rb_scene_create(const rb_scene_desc* desc, rb_scene** out) {
         meshes[s].vertices.assign(sc->shapes[s].vertices, sc->shapes[s].vertices + 3 * (size_t)sc->shapes[s].num_vertices);
         meshes[s].indices.assign(sc->shapes[s].indices, sc->shapes[s].indices + 3 * (size_t)sc->shapes[s].num_triangles);
     }
-    d.num_lights = (int)sc->lights.size();
-    d.has_envmap = desc->envmap != nullptr;
-    if (d.has_envmap) {
-        const rb_envmap& e = *desc->envmap;
-        d.env.values = e.values;
-        memcpy(d.env.w2e, e.world_to_env, sizeof(d.env.w2e));
-        memcpy(d.env.e2w, e.env_to_world, sizeof(d.env.e2w));
-        d.env.cdf_ys = e.sample_cdf_ys;
-        d.env.cdf_xs = e.sample_cdf_xs;
-        d.env.pdf_norm = e.pdf_norm;
-        d.env.directly_visible = e.directly_visible;
-        d.num_lights++;
-    }
+    host_setup_envmap(desc->envmap, d);
+    d.num_lights = (int)sc->lights.size() + (d.has_envmap ? 1 : 0);
     if (d.num_lights > 0) {
         if (!host_build_lights(sc->lights, meshes, sc->lt, g_err, d.has_envmap != 0, d.has_envmap ? desc->envmap->pdf_norm : 0.0, host_bsphere_radius(meshes))) return 1;
         d.lights = sc->lights.data();
@@ -239,69 +224,35 @@ extern "C" int rb_scene_last_stats(const rb_scene*, int* n, float* ms) {
 
 extern "C" int rb_render(const rb_scene* scene, const rb_options* opt, float* image, const float* d_image, const rb_dscene_desc* d_scene,
                          float* screen_grad, void*) {
-    KernelArgs ka;
-    memset(&ka, 0, sizeof(ka));
-    RenderParams& rp = ka.rp;
-    rp.seed = opt->seed;
-    rp.spp = opt->num_samples;
-    rp.max_bounces = opt->max_bounces;
-    rp.sampler_type = opt->sampler_type;
-    rp.sample_pixel_center = opt->sample_pixel_center;
-    rp.num_channels = opt->num_channels;
-    rp.rad_dim = -1;
-    for (int i = 0; i < opt->num_channels; i++)
-        if (opt->channels[i] == RB_CH_RADIANCE) rp.rad_dim = i;
-    rp.nd = host_compute_num_channels(opt->channels, opt->num_channels, scene->max_generic);
-    rp.rad_off = -1;
-    for (int i = 0, off = 0; i < opt->num_channels; i++) {
-        if (opt->channels[i] == RB_CH_RADIANCE) rp.rad_off = off;
-        off += rb_channel_width(opt->channels[i], scene->max_generic);
+    if (!scene || !opt) {
+        g_err = "rb_render: null scene / options";
+        return 1;
     }
-    rp.part = scene->part; rp.num_parts = scene->num_parts; rp.rows_per_stripe = scene->rps; // round-robin stripes of rows, as in rb_kernels_body.cuh
-    auto owned = [&](int y) { return (y / rp.rows_per_stripe) % rp.num_parts == rp.part; };
-    rp.vp_w = scene->cam.viewport_end[0] - scene->cam.viewport_beg[0];
-    rp.vp_h = scene->cam.viewport_end[1] - scene->cam.viewport_beg[1];
-    ka.lanes_per_pixel = 1;
-    while (ka.lanes_per_pixel * 2 <= std::min(32, rp.spp)) ka.lanes_per_pixel *= 2;
-    ka.image = image;
-    ka.d_image = d_image;
-    ka.screen_grad = screen_grad;
+    KernelArgs ka;
+    if (const char* err = setup_kernel_args(*opt, scene->cam, scene->max_generic, scene->part, scene->num_parts, scene->rps, image, d_image, d_scene,
+                                            screen_grad, ka)) {
+        g_err = err;
+        return 1;
+    }
+    const RenderParams& rp = ka.rp;
+    if (rp.vp_w <= 0 || rp.vp_h <= 0 || rp.spp == 0) return 0;
     const DevScene& sc = scene->dev;
-    for (int i = 0; i < opt->num_channels; i++) rp.channels[i] = opt->channels[i];
-    rp.max_generic = scene->max_generic;
-    bool only_radiance = opt->num_channels == 1 && opt->channels[0] == RB_CH_RADIANCE;
-    rp.only_radiance = only_radiance ? 1 : 0;
-    if (image && !only_radiance) {
-        for (int y = 0; y < rp.vp_h; y++)
+    if (image && !rp.only_radiance) {
+        for (int j = 0; j < ka.owned_rows; j++)
             for (int x = 0; x < rp.vp_w; x++) {
-                if (!owned(y)) continue;
-                int pixel = y * rp.vp_w + x;
+                const int y = owned_row_to_row(rp, j), pixel = y * rp.vp_w + x;
                 float acc[RB_MAX_ND] = {0};
                 int ids[3] = {-1, -1, -1}, last = -1;
                 for (int s = 0; s < rp.spp; s++) {
                     int cur[3] = {-1, -1, -1};
                     if (forward_sample_channels(sc, rp, pixel, x, y, s, acc, cur)) { last = s; ids[0] = cur[0]; ids[1] = cur[1]; ids[2] = cur[2]; }
                 }
-                float* px = image + (size_t)rp.nd * pixel;
-                int d = 0;
-                for (int c = 0; c < rp.num_channels; c++) {
-                    int ch = rp.channels[c];
-                    int width = (ch == RB_CH_RADIANCE || ch == RB_CH_POSITION || ch == RB_CH_GEOMETRY_NORMAL || ch == RB_CH_SHADING_NORMAL ||
-                                 ch == RB_CH_DIFFUSE_REFLECTANCE || ch == RB_CH_SPECULAR_REFLECTANCE || ch == RB_CH_VERTEX_COLOR) ? 3
-                              : (ch == RB_CH_UV || ch == RB_CH_BARYCENTRIC) ? 2 : (ch == RB_CH_GENERIC_TEXTURE ? rp.max_generic : 1);
-                    if (ch == RB_CH_SHAPE_ID || ch == RB_CH_TRIANGLE_ID || ch == RB_CH_MATERIAL_ID) {
-                        if (last >= 0) px[d] = (float)ids[ch - RB_CH_SHAPE_ID];
-                    } else {
-                        for (int i = 0; i < width; i++) px[d + i] += acc[d + i];
-                    }
-                    d += width;
-                }
+                write_gbuffer_pixel(rp, acc, ids, last >= 0, image + (size_t)rp.nd * pixel);
             }
     } else if (image) {
-        for (int y = 0; y < rp.vp_h; y++)
+        for (int j = 0; j < ka.owned_rows; j++)
             for (int x = 0; x < rp.vp_w; x++) {
-                if (!owned(y)) continue;
-                int pixel = y * rp.vp_w + x;
+                const int y = owned_row_to_row(rp, j), pixel = y * rp.vp_w + x;
                 V3 acc = zero3();
                 for (int s = 0; s < rp.spp; s++) acc += forward_sample(sc, rp, pixel, x, y, s);
                 float* px = image + (size_t)rp.nd * pixel + rp.rad_dim;
@@ -309,18 +260,16 @@ extern "C" int rb_render(const rb_scene* scene, const rb_options* opt, float* im
             }
     }
     if (d_image) {
+        if (const char* err = setup_backward(*d_scene, sc, ka)) {
+            g_err = err;
+            return 1;
+        }
         std::vector<double> cam_accum(RB_CAM_ACC, 0.0);
         std::vector<float> cam_f(RB_CAM_ACC, 0.f);
         ka.ds.shapes = d_scene->shapes;
         ka.ds.materials = d_scene->materials;
         ka.ds.light_intensity = d_scene->light_intensity;
         ka.ds.cam_accum = cam_accum.data();
-        memset(&ka.ds.env_values, 0, sizeof(rb_texture));
-        ka.ds.env_w2e = nullptr;
-        if (d_scene->envmap != nullptr) {
-            ka.ds.env_values = d_scene->envmap->values;
-            ka.ds.env_w2e = d_scene->envmap->world_to_env;
-        }
         CamAcc acc;
         acc.base = cam_f.data();
         acc.stride = 1;
@@ -338,17 +287,17 @@ extern "C" int rb_render(const rb_scene* scene, const rb_options* opt, float* im
             }
         }
 #endif
-        for (int y = 0; y < rp.vp_h; y++)
+        for (int j = 0; j < ka.owned_rows; j++)
             for (int x = 0; x < rp.vp_w; x++)
                 for (int s = 0; s < rp.spp; s++) {
-                    if (!owned(y)) continue;
+                    const int y = owned_row_to_row(rp, j);
 #ifdef RB_EMU_REF_STREAMS
                     rb_emu_rank = &ranks[((size_t)s * npx + (size_t)y * rp.vp_w + x) * mbr];
 #endif
                     backward_sample(sc, ka, y * rp.vp_w + x, x, y, s, recs.data(), acc);
                     for (int k = 0; k < RB_CAM_ACC; k++) { cam_accum[k] += cam_f[k]; cam_f[k] = 0.f; }
                 }
-        if (sc.use_primary_edge && sc.num_edges > 0) {
+        if (primary_edge_pass_runs(sc)) {
             long long n_px = (long long)rp.vp_w * rp.vp_h;
             for (long long i = 0; i < n_px; i++)
                 for (int s = 0; s < rp.spp; s++) {
