@@ -52,7 +52,9 @@ def build(force=False, double=False, verbose=False, defines=(), out=None, nvcc_f
     if verbose:
         common += ["-Xptxas", "-v"]
     # rb_edge_tree.cu builds the secondary-edge trees and must round like the host builder it is tested against (no FMA contraction,
-    # IEEE division / square root); its bottom-up passes hand data between thread blocks, so its global loads bypass the L1.
+    # IEEE division / square root); its bottom-up passes hand data between thread blocks, so its global loads bypass the L1.  The
+    # steps it shares with the host builder are header-only (rb_edge_tree.cuh) so that they are compiled inside this translation unit,
+    # under these flags, rather than in an object built with the fast ones.
     # rb_edge_list.cu drops coplanar edges by a threshold on a dot product of unit normals: same rounding rule.
     per_file = {"rb_edge_tree.cu": ["-fmad=false", "-prec-div=true", "-prec-sqrt=true", "-Xptxas", "-dlcm=cg"],
                 "rb_edge_list.cu": ["-fmad=false", "-prec-div=true", "-prec-sqrt=true"]}

@@ -102,3 +102,14 @@ RB_HD bool clip_line_unit(V2 v0, V2 v1, V2& a, V2& b) {
     }
     return false;
 }
+
+// Weight of an edge in the primary-edge distribution (src/edge.cpp:186-214): its screen-space length after clipping to the image if
+// it is a silhouette seen from the camera, else 0.
+RB_HD double primary_edge_weight(const DevCamera& cam, const rb_shape* shapes, const Edge& e) {
+    double iw = 1.0 / cam.c2w[15];
+    V3 org = mk3((Real)(cam.c2w[3] * iw), (Real)(cam.c2w[7] * iw), (Real)(cam.c2w[11] * iw));
+    V3 v0 = edge_v0(shapes, e), v1 = edge_v1(shapes, e);
+    V2 p0, p1, c0, c1;
+    if (cam_project(cam, v0, v1, p0, p1) && clip_line_unit(p0, p1, c0, c1) && edge_is_silhouette(shapes, org, e)) return length(c1 - c0);
+    return 0;
+}

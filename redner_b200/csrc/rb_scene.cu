@@ -97,15 +97,6 @@ __global__ void k_scene_bounds(const rb_shape* shapes, const int* tri_offset, in
         }
     }
 }
-__device__ __forceinline__ unsigned long long expand21(unsigned int v) {
-    unsigned long long x = v & 0x1fffffu;
-    x = (x | x << 32) & 0x1f00000000ffffULL;
-    x = (x | x << 16) & 0x1f0000ff0000ffULL;
-    x = (x | x << 8) & 0x100f00f00f00f00fULL;
-    x = (x | x << 4) & 0x10c30c30c30c30c3ULL;
-    x = (x | x << 2) & 0x1249249249249249ULL;
-    return x;
-}
 __global__ void k_morton(const rb_shape* shapes, const int* tri_offset, int num_shapes, int T, const unsigned int* bounds,
                          unsigned long long* keys, int* vals) {
     int g = blockIdx.x * blockDim.x + threadIdx.x;
