@@ -177,6 +177,30 @@ int rb_scene_create(const rb_scene_desc* desc, rb_scene** out);
  * mesh read-back and build kernels are ordered after the work already queued on that stream -- pass the stream the geometry tensors
  * were produced on.  rb_scene_set_camera and rb_scene_destroy keep using it. */
 int rb_scene_create_on_stream(const rb_scene_desc* desc, rb_scene** out, void* stream);
+/* Re-target an existing scene at a descriptor of the SAME structure, without building a new scene (an optimisation step that moves
+ * vertices or changes materials, lights or the camera).  The structure is:
+ *   - the numbers of shapes, materials and lights;
+ *   - per shape: num_vertices, num_triangles, num_uv_vertices, num_normal_vertices, material_id, light_id, and which optional
+ *     buffers (uvs, normals, uv_indices, normal_indices, colors) are present;
+ *   - per light: shape_id;
+ *   - the presence of the environment map, both edge-sampling flags, gpu_index and the largest generic texture dimension.
+ * All of it is checked before any work; on a mismatch the call fails with a message and the scene is left unchanged and usable.
+ * The CONTENTS of every index buffer must be those of the build as well: the caller promises this, the library does not check it.
+ * Any pointer may change, and so may every value passed by value (camera, light intensities, the environment map's matrices and
+ * pdf_norm).
+ * The build reads vertex positions in place, so an in-place write to them is invisible to the library: pass geometry_changed != 0
+ * after one.  Then -- or when any `vertices` pointer changed -- the BVH, the light areas and area CDFs, the environment map's
+ * bounding sphere, the edge list and the camera-dependent tables are rebuilt.  Otherwise, when the camera differs by value, only the
+ * camera-dependent tables are, as rb_scene_set_camera does (but on the host for the small scenes whose build made them there, so
+ * that they stay the build's tables byte for byte).  The shape / material descriptors, the lights and the light PMF / CDF are
+ * refreshed on every call.
+ * After a successful update every table of the scene is the one rb_scene_create would build from the same descriptor, byte for
+ * byte.  `stream` becomes the scene's stream (as with rb_scene_create_on_stream), rb_scene_build_ms reports this update and the
+ * partition of rb_scene_set_partition is kept.  After rb_scene_set_camera on a scene whose build made the camera-dependent tables on
+ * the host, the next update makes them on the host again.  A failure after the checks (a BVH too deep for the traversal stack, a
+ * total light importance that is not positive, a device error) leaves the scene incomplete: rb_render and rb_scene_set_camera refuse
+ * it, and the next rb_scene_update rebuilds every table whatever geometry_changed says. */
+int rb_scene_update(rb_scene* scene, const rb_scene_desc* desc, int geometry_changed, void* stream);
 void rb_scene_destroy(rb_scene* scene);
 /* Scene::max_generic_texture_dimension (src/scene.cpp:293-300, bound at src/redner.cpp:72) */
 int rb_scene_max_generic_texture_dimension(const rb_scene* scene);
@@ -225,7 +249,7 @@ int rb_scene_last_backward_stats(const rb_scene* scene, float* bwd_ms3);
 /* rb_render keeps one grow-only scratch allocation per device for the backward pass (gradient descriptors, path
  * records, work lists; at most ~1 GiB + small).  This frees them all; the next backward pass allocates again. */
 void rb_release_scratch(void);
-/* Host wall-clock milliseconds rb_scene_create spent in { BVH build, light tables, edge list + edge tree }. */
+/* Host wall-clock milliseconds the last rb_scene_create or rb_scene_update spent in { BVH build, light tables, edge list + edge tree }. */
 int rb_scene_build_ms(const rb_scene* scene, float* bvh_lights_edges3);
 
 /* Test hook: the secondary-edge trees as the kernels see them.  info3 = { number of 128-byte records, root reference of the
@@ -235,6 +259,21 @@ int rb_scene_edge_trees(const rb_scene* scene, int* info3, float* expand, void* 
 /* Test hook: the scene's edge list (what collect_edges builds, src/edge.cpp:233-296): *num_edges, and up to edges_bytes of
  * { shape, v0, v1, f0, f1 } int records into edges_out (may be NULL). */
 int rb_scene_edge_list(const rb_scene* scene, int* num_edges, int* edges_out, size_t edges_bytes);
+
+/* Test hook: one table of the scene as the kernels see it.  *size (may be NULL) receives its size in bytes; out (may be NULL) receives
+ * up to `bytes` of it. */
+enum rb_scene_table_id {
+    RB_TABLE_BVH_NODES = 0,      /* triangle BVH inner nodes (scene triangles - 1 of them) */
+    RB_TABLE_BVH_TRIANGLES,      /* triangles in BVH leaf order */
+    RB_TABLE_LIGHT_PMF,          /* double per light, the environment map last (src/scene.cpp:197-253) */
+    RB_TABLE_LIGHT_CDF,
+    RB_TABLE_LIGHT_AREAS,        /* double per area light */
+    RB_TABLE_AREA_CDF_POOL,      /* double per emissive triangle: every light's triangle-area CDF */
+    RB_TABLE_AREA_CDF_OFFSETS,   /* int per area light: first entry in the pool */
+    RB_TABLE_PRIMARY_EDGE_PMF,   /* double per edge (src/edge.cpp:298-331); empty without primary-edge sampling */
+    RB_TABLE_PRIMARY_EDGE_CDF
+};
+int rb_scene_table(const rb_scene* scene, int which, void* out, size_t bytes, size_t* size);
 
 const char* rb_last_error(void);
 const char* rb_version(void);

@@ -16,6 +16,10 @@ RB_MAX_MIP_LEVELS = 8
 c_float_p = C.POINTER(C.c_float)
 c_int_p = C.POINTER(C.c_int)
 
+# enum rb_scene_table_id
+RB_TABLES = ("bvh_nodes", "bvh_triangles", "light_pmf", "light_cdf", "light_areas", "area_cdf_pool", "area_cdf_offsets", "primary_edge_pmf",
+             "primary_edge_cdf")
+
 
 class rb_camera(C.Structure):
     _fields_ = [
@@ -110,7 +114,7 @@ class rb_dscene_desc(C.Structure):
 
 EXPORTS = [
     "rb_scene_create", "rb_scene_create_on_stream", "rb_scene_destroy", "rb_scene_max_generic_texture_dimension", "rb_compute_num_channels", "rb_render",
-    "rb_scene_set_partition", "rb_scene_last_stats", "rb_scene_last_stage_stats", "rb_scene_last_backward_stats", "rb_release_scratch", "rb_scene_build_ms", "rb_scene_edge_trees", "rb_scene_edge_list", "rb_scene_set_camera", "rb_render_batch", "rb_last_error", "rb_version",
+    "rb_scene_set_partition", "rb_scene_last_stats", "rb_scene_last_stage_stats", "rb_scene_last_backward_stats", "rb_release_scratch", "rb_scene_build_ms", "rb_scene_edge_trees", "rb_scene_edge_list", "rb_scene_table", "rb_scene_set_camera", "rb_scene_update", "rb_render_batch", "rb_last_error", "rb_version",
 ]
 
 
@@ -120,6 +124,9 @@ def _bind(lib):
     if hasattr(lib, "rb_scene_create_on_stream"):
         lib.rb_scene_create_on_stream.argtypes = [C.POINTER(rb_scene_desc), C.POINTER(C.c_void_p), C.c_void_p]
         lib.rb_scene_create_on_stream.restype = C.c_int
+    if hasattr(lib, "rb_scene_update"):
+        lib.rb_scene_update.argtypes = [C.c_void_p, C.POINTER(rb_scene_desc), C.c_int, C.c_void_p]
+        lib.rb_scene_update.restype = C.c_int
     lib.rb_scene_destroy.argtypes = [C.c_void_p]
     lib.rb_scene_destroy.restype = None
     lib.rb_scene_max_generic_texture_dimension.argtypes = [C.c_void_p]
@@ -156,6 +163,9 @@ def _bind(lib):
     if hasattr(lib, "rb_scene_edge_list"):
         lib.rb_scene_edge_list.argtypes = [C.c_void_p, c_int_p, c_int_p, C.c_size_t]
         lib.rb_scene_edge_list.restype = C.c_int
+    if hasattr(lib, "rb_scene_table"):
+        lib.rb_scene_table.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
+        lib.rb_scene_table.restype = C.c_int
     lib.rb_last_error.argtypes = []
     lib.rb_last_error.restype = C.c_char_p
     lib.rb_version.argtypes = []

@@ -279,9 +279,10 @@ class RenderFunction(torch.autograd.Function):
         return args
 
     @staticmethod
-    def _unpack(seed, args, scene=None):
+    def _unpack(seed, args, scene=None, geometry_changed=None):
         """`scene`: an existing native scene of the SAME geometry / materials / lights to re-target at this argument list's camera
-        (rb_scene_set_camera) instead of building a new one -- the batch path."""
+        (rb_scene_set_camera) instead of building a new one -- the batch path.  With `geometry_changed` (True / False) the scene only
+        needs the same structure and is re-targeted at everything in the argument list (Scene.update) -- the SceneRenderer path."""
         it = iter(args)
         nxt = lambda: next(it)  # noqa: E731
         c = _Ctx()
@@ -345,6 +346,9 @@ class RenderFunction(torch.autograd.Function):
         c.env_args, c.envmap = env_args, envmap
         if scene is None:
             c.scene = rb.Scene(camera, shapes, materials, lights, envmap, use_gpu, gpu_index, use_prim, use_sec)
+        elif geometry_changed is not None:
+            scene.update(camera, shapes, materials, lights, envmap, geometry_changed=geometry_changed)
+            c.scene = scene
         else:
             scene.set_camera(camera)
             c.scene = scene
@@ -488,6 +492,127 @@ class BatchRenderFunction(torch.autograd.Function):
             one.c, one.args = c, ctx.args[k * ctx.n:(k + 1) * ctx.n]
             out += list(RenderFunction.backward(one, grad_imgs[k]))[1:]
         return tuple(out)
+
+
+class SceneRenderer:
+    """Renders one scene over and over -- the steps of an optimisation loop -- through ONE native scene that is updated in place
+    (Scene.update / rb_scene_update) instead of built anew for every call the way RenderFunction does.
+
+        render = SceneRenderer(num_samples, max_bounces, **serialize_scene options)
+        img = render(scene, seed)   # RenderFunction.apply(seed, *serialize_scene(scene, ...)), with autograd
+
+    The first call builds the native scene.  A later call whose scene has the same structure (shapes, vertex / triangle counts,
+    material and light ids, optional buffers, lights, environment map, and the edge-sampling flags, which follow `requires_grad`)
+    updates it: the BVH, light areas and edge list are rebuilt only when a vertex tensor was replaced or written to in place (its
+    `_version`); a material, light intensity or camera change refreshes the light PMF and the camera tables alone.  An index tensor that
+    was replaced or written to is compared with a copy of the one the scene was built from; a change there, or any other change of
+    structure, builds a new native scene.  Images are those of RenderFunction; the backward pass renders against the state its forward
+    pass saw, even if the scene has been updated since."""
+
+    def __init__(self, num_samples, max_bounces: int, **options):
+        self.num_samples, self.max_bounces, self.options = num_samples, max_bounces, options
+        self._scene = None       # the native scene
+        self._key = None         # structure of its last descriptor
+        self._vertices = None    # [(vertex tensor, its _version)] of the last descriptor
+        self._indices = None     # [(index tensor, its _version, copy)] of the build
+
+    @staticmethod
+    def _structure(args):
+        """The parts of a serialize_scene list that rb_scene_update requires to be unchanged, except the contents of index buffers."""
+        it = iter(args)
+        nxt = lambda: next(it)  # noqa: E731
+        num_shapes, num_materials, num_lights = nxt(), nxt(), nxt()
+        for _ in range(12):
+            nxt()
+        shapes, mats, lights = [], [], []
+        for _ in range(num_shapes):
+            v, i, uv, n, uvi, ni, col, mid, lid = [nxt() for _ in range(9)]
+            shapes.append((tuple(v.shape), tuple(i.shape), tuple(uv.shape) if uv is not None else None, tuple(n.shape) if n is not None else None,
+                           uvi is not None, ni is not None, col is not None, int(mid), int(lid)))
+        for _ in range(num_materials):
+            texs = []
+            for _ in range(5):
+                k = nxt()
+                texs.append(None if k == 0 else tuple(tuple(nxt().shape) for _ in range(k + 1)))  # (mip levels, then uv_scale)
+            mats.append((tuple(texs), nxt(), nxt(), nxt()))
+        for _ in range(num_lights):
+            lights.append(int(nxt()))
+            nxt(), nxt(), nxt()
+        k = nxt()
+        env = None if k is None else tuple(tuple(nxt().shape) for _ in range(k + 1))  # (mip levels, then uv_scale)
+        if k is not None:
+            for _ in range(6):  # matrices, sampling tables, pdf_norm, directly_visible
+                nxt()
+        rest = [nxt() for _ in range(9)]
+        flags = (bool(rest[4]), bool(rest[5]), str(rest[7]))  # edge-sampling flags, device
+        return tuple(shapes), tuple(mats), tuple(lights), env, flags
+
+    def _target(self, args):
+        """(geometry_changed, state): geometry_changed is None to build a new native scene for `args`, else the flag for an update of the
+        current one; `state` is what _commit records once the native call has succeeded."""
+        key = self._structure(args)
+        n = args[0]
+        verts = [args[15 + 9 * s] for s in range(n)]
+        inds = [args[16 + 9 * s] for s in range(n)]
+        fresh = self._scene is None or key != self._key
+        if not fresh:
+            for t, (t0, ver0, copy) in zip(inds, self._indices):
+                if (t is not t0 or t._version != ver0) and not torch.equal(t, copy):
+                    fresh = True
+                    break
+        if fresh:
+            indices = [(t, t._version, t.clone()) for t in inds]
+            geometry = None
+        else:
+            indices = [(t, t._version, copy) for t, (_, _, copy) in zip(inds, self._indices)]
+            geometry = any(t is not t0 or t._version != ver0 for t, (t0, ver0) in zip(verts, self._vertices))
+        return geometry, (key, [(t, t._version) for t in verts], indices)
+
+    def _commit(self, scene, state):
+        self._scene = scene
+        self._key, self._vertices, self._indices = state
+
+    def _forget(self):
+        """After a failed build or update: the next call builds a new native scene."""
+        self._scene = self._key = self._vertices = self._indices = None
+
+    def __call__(self, scene: Scene, seed):
+        args = RenderFunction.serialize_scene(scene, self.num_samples, self.max_bounces, **self.options)
+        return _SceneRenderFunction.apply(seed, self, *args)
+
+
+class _SceneRenderFunction(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, seed, renderer, *args):
+        assert isinstance(seed, (tuple, int))
+        if not isinstance(seed, tuple):
+            seed = (seed, seed if _use_correlated_random_number else seed + 1000003)
+        geometry, state = renderer._target(args)
+        try:
+            c = RenderFunction._unpack(seed, args, scene=renderer._scene if geometry is not None else None, geometry_changed=geometry)
+        except Exception:
+            renderer._forget()
+            raise
+        renderer._commit(c.scene, state)
+        c.scene._generation = getattr(c.scene, "_generation", 0) + 1
+        ctx.generation = c.scene._generation
+        rb = c.backend
+        nch = rb.compute_num_channels(c.channels, c.scene.max_generic_texture_dimension)
+        h, w = c.viewport[2] - c.viewport[0], c.viewport[3] - c.viewport[1]
+        img = torch.zeros(h, w, nch, device=c.device)
+        rb.render(c.scene, c.options, rb.float_ptr(img.data_ptr()), rb.float_ptr(0), None, rb.float_ptr(0), rb.float_ptr(0))
+        ctx.c = c
+        ctx.args = args  # keeps the tensors alive (the native side only holds raw pointers)
+        return img
+
+    @staticmethod
+    def backward(ctx, grad_img):
+        c = ctx.c
+        if c.scene._generation != ctx.generation:  # updated since this forward pass: back to the state it rendered
+            c.scene.update(c.camera, c.shapes, c.materials, c.lights, c.envmap, geometry_changed=True)
+            c.scene._generation += 1
+            ctx.generation = c.scene._generation
+        return (None,) + RenderFunction.backward(ctx, grad_img)
 
 
 def render_batch(scenes, num_samples, max_bounces: int, seeds, **kw) -> torch.Tensor:

@@ -56,8 +56,10 @@ def build(force=False, double=False, verbose=False, defines=(), out=None, nvcc_f
     # steps it shares with the host builder are header-only (rb_edge_tree.cuh) so that they are compiled inside this translation unit,
     # under these flags, rather than in an object built with the fast ones.
     # rb_edge_list.cu drops coplanar edges by a threshold on a dot product of unit normals: same rounding rule.
+    # rb_light_build.cu computes the light tables in double with the steps of the host builder (rb_light_build.cuh): same rounding rule.
     per_file = {"rb_edge_tree.cu": ["-fmad=false", "-prec-div=true", "-prec-sqrt=true", "-Xptxas", "-dlcm=cg"],
-                "rb_edge_list.cu": ["-fmad=false", "-prec-div=true", "-prec-sqrt=true"]}
+                "rb_edge_list.cu": ["-fmad=false", "-prec-div=true", "-prec-sqrt=true"],
+                "rb_light_build.cu": ["-fmad=false", "-prec-div=true", "-prec-sqrt=true"]}
     objs = []
     procs = []
     for src in sorted(glob.glob(os.path.join(CSRC, "*.cu"))):

@@ -130,11 +130,13 @@ int rb_build_edge_list_gpu(rb_scene* sc, cudaStream_t stream) {
     RB_CUDA_OK(cudaStreamSynchronize(stream));
     if (E < 0 || E > M) return fail("edge list: inconsistent edge count");
     if (E > 0) {
-        void* edges = nullptr;
-        if (cudaMallocAsync(&edges, sizeof(Edge) * (size_t)E, stream) != cudaSuccess) return fail("out of device memory for the edge list");
-        sc->allocs.push_back(edges);
-        k_el_compact<<<GM, B, 0, stream>>>(M, paired, flags, ranks, (Edge*)edges);
-        sc->dev.edges = (Edge*)edges;
+        Edge* edges = nullptr;
+        if (scene_table(sc, SS_EDGES, E, stream, &edges)) {
+            release();
+            return 1;
+        }
+        k_el_compact<<<GM, B, 0, stream>>>(M, paired, flags, ranks, edges);
+        sc->dev.edges = edges;
     }
     sc->dev.num_edges = E;
     RB_CUDA_OK(cudaGetLastError());

@@ -310,6 +310,8 @@ int rb_build_edge_trees_gpu(rb_scene* sc, cudaStream_t stream) {
     auto release = [&]() {
         for (void* p : temps) cudaFreeAsync(p, stream);
     };
+    EdgeNode* out = nullptr; // (kept across rebuilds while the number of edges stays the same)
+    if (scene_table(sc, SS_EDGE_NODES, E, stream, &out)) return 1;
     ETNode* leaves = (ETNode*)talloc(sizeof(ETNode) * (size_t)E);
     ETNode* nodes = (ETNode*)talloc(sizeof(ETNode) * (2 * (size_t)E + 2));
     unsigned char* is_cs = (unsigned char*)talloc(E);
@@ -320,16 +322,10 @@ int rb_build_edge_trees_gpu(rb_scene* sc, cudaStream_t stream) {
     size_t sort_bytes = 0;
     cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, keys, keys_sorted, vals, ids, E, 0, 64, stream);
     void* sort_tmp = talloc(sort_bytes);
-    EdgeNode* out = sc->edge_nodes_buf; // (reused when rb_scene_set_camera rebuilds the trees: the edge list does not change)
-    if (!leaves || !nodes || !is_cs || !g || !keys || !keys_sorted || !vals || !ids || !counters || !sort_tmp ||
-        (out == nullptr && cudaMallocAsync((void**)&out, sizeof(EdgeNode) * (size_t)std::max(E, 1), stream) != cudaSuccess)) {
+    if (!leaves || !nodes || !is_cs || !g || !keys || !keys_sorted || !vals || !ids || !counters || !sort_tmp) {
         release();
         rb_set_error("rb_scene_create: out of device memory for the edge trees");
         return 1;
-    }
-    if (sc->edge_nodes_buf == nullptr) {
-        sc->allocs.push_back(out);
-        sc->edge_nodes_buf = out;
     }
     ETGlobals g0;
     memset(&g0, 0, sizeof(g0));
@@ -408,17 +404,10 @@ __global__ void k_prim_normalize(int E, const double* total, double* pmf) {
 int rb_build_primary_edge_cdf_gpu(rb_scene* sc, cudaStream_t stream) {
     const int E = sc->dev.num_edges;
     if (E == 0 || !sc->dev.use_primary_edge) return 0;
-    double *pmf = const_cast<double*>(sc->dev.prim_edge_pmf), *cdf = const_cast<double*>(sc->dev.prim_edge_cdf);
-    if (pmf == nullptr || cdf == nullptr) {
-        if (cudaMallocAsync((void**)&pmf, sizeof(double) * (size_t)E, stream) != cudaSuccess || cudaMallocAsync((void**)&cdf, sizeof(double) * (size_t)E, stream) != cudaSuccess) {
-            rb_set_error("rb_scene_create: out of device memory for the primary-edge distribution");
-            return 1;
-        }
-        sc->allocs.push_back(pmf);
-        sc->allocs.push_back(cdf);
-        sc->dev.prim_edge_pmf = pmf;
-        sc->dev.prim_edge_cdf = cdf;
-    }
+    double *pmf = nullptr, *cdf = nullptr; // (kept across rebuilds while the number of edges stays the same)
+    if (scene_table(sc, SS_PRIM_PMF, E, stream, &pmf) || scene_table(sc, SS_PRIM_CDF, E, stream, &cdf)) return 1;
+    sc->dev.prim_edge_pmf = pmf;
+    sc->dev.prim_edge_cdf = cdf;
     size_t b1 = 0, b2 = 0;
     cub::DeviceReduce::Sum(nullptr, b1, pmf, (double*)nullptr, E, stream);
     cub::DeviceScan::ExclusiveSum(nullptr, b2, pmf, cdf, E, stream);

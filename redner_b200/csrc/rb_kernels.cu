@@ -104,6 +104,10 @@ extern "C" int rb_render(const rb_scene* scene_, const rb_options* opt, float* i
         rb_set_error("rb_render: null scene / options");
         return 1;
     }
+    if (scene->incomplete) {
+        rb_set_error("rb_render: the scene's last update failed; update it again or build a new scene");
+        return 1;
+    }
     KernelArgs ka;
     if (const char* err = setup_kernel_args(*opt, scene->cam, scene->max_generic_texture_dimension, scene->part, scene->num_parts, scene->rows_per_stripe,
                                             image, d_image, d_scene, screen_grad, ka)) {

@@ -26,16 +26,29 @@ struct EventPool {
     }
 };
 
+// Device tables owned by a scene, one slot each.  scene_table() keeps a slot's buffer when the requested size is unchanged and otherwise
+// frees it in stream order and allocates a new one, so an update that rebuilds a table replaces it instead of adding to it.
+enum SceneSlot {
+    SS_SHAPES, SS_MATERIALS, SS_BVH_NODES, SS_BVH_TRIS, SS_LIGHTS, SS_LIGHT_PMF, SS_LIGHT_CDF, SS_LIGHT_AREAS, SS_AREA_POOL, SS_AREA_OFFSETS,
+    SS_LIGHT_AUX, SS_EDGES, SS_PRIM_PMF, SS_PRIM_CDF, SS_EDGE_NODES, SS_COUNT
+};
+struct SceneBuffer {
+    void* p = nullptr;
+    size_t bytes = 0;
+};
+
 struct rb_scene {
     int device = 0;
-    cudaStream_t stream = 0; // stream of rb_scene_create_on_stream: builds, rb_scene_set_camera and the frees of rb_scene_destroy
+    int gpu_index = -1;      // as in the descriptor of the build
+    cudaStream_t stream = 0; // stream of the last build or update: builds, rb_scene_set_camera and the frees of rb_scene_destroy
     EventPool events;
     DevScene dev;   // passed by value to kernels
     rb_camera cam;  // host copy of the descriptor camera
-    std::vector<void*> allocs; // device allocations owned by the scene
+    SceneBuffer bufs[SS_COUNT]; // device tables owned by the scene
     std::vector<rb_shape> shapes;
     std::vector<rb_material> materials;
     std::vector<DevLight> lights;
+    std::vector<int> light_offsets; // [lights + 1]: first entry of every light in the area-CDF pool, then the pool size
     int max_generic_texture_dimension = 0;
     int has_envmap = 0;
     // partition (multi-GPU)
@@ -48,8 +61,11 @@ struct rb_scene {
     double last_path_vertices = 0, last_primary_hits = 0;
     int num_edge_nodes = 0; // records of the secondary-edge trees (dev.edge_nodes)
     bool edge_list_on_device = false;   // this scene's edge list was built by rb_edge_list.cu (else on the host)
-    EdgeNode* edge_nodes_buf = nullptr; // device buffer of the GPU tree builder (num_edges records), reused by rb_scene_set_camera
-    // scene-build timings (ms, host clock) for reporting
+    bool host_tables = false;           // ... and its camera-dependent tables on the host, from host_edges
+    bool camera_tables_as_built = true; // the camera-dependent tables are on the side the build chose (not rb_scene_set_camera's device)
+    bool incomplete = false;            // the last build / update / camera change failed part-way: rb_render refuses the scene
+    std::vector<Edge> host_edges;
+    // timings of the last build or update (ms, host clock) for reporting
     float build_ms_bvh = 0.f, build_ms_lights = 0.f, build_ms_edges = 0.f;
 };
 
@@ -70,8 +86,18 @@ extern "C" const unsigned char rb_sobol_table_end[];
 extern "C" const unsigned char rb_ltc_table_begin[];
 extern "C" const unsigned char rb_ltc_table_end[];
 
+int scene_buffer(rb_scene* sc, SceneSlot slot, size_t bytes, cudaStream_t stream, void** out); // rb_scene.cu
+template <typename T>
+int scene_table(rb_scene* sc, SceneSlot slot, size_t count, cudaStream_t stream, T** out) {
+    void* p = nullptr;
+    if (scene_buffer(sc, slot, (count > 0 ? count : 1) * sizeof(T), stream, &p)) return 1;
+    *out = (T*)p;
+    return 0;
+}
+
 int rb_build_bvh(rb_scene* sc, cudaStream_t stream);
-int rb_build_lights(rb_scene* sc, cudaStream_t stream);
+int rb_build_lights(rb_scene* sc, bool geometry, cudaStream_t stream); // rb_light_build.cu
+int rb_light_status(const rb_scene* sc, cudaStream_t stream, int* status);
 int rb_build_edges(rb_scene* sc, cudaStream_t stream);
 int rb_build_edge_list_gpu(rb_scene* sc, cudaStream_t stream);  // rb_edge_list.cu
 int rb_build_edge_trees_gpu(rb_scene* sc, cudaStream_t stream); // rb_edge_tree.cu

@@ -312,19 +312,6 @@ class Scene:  # src/redner.cpp:62-73, src/scene.cpp:63-307
         lib = L.load()
         self._lib = lib
         self._handle = None
-        d = L.rb_scene_desc()
-        d.camera = camera._c
-        self._shapes = (L.rb_shape * max(1, len(shapes)))(*[s._c for s in shapes])
-        self._materials = (L.rb_material * max(1, len(materials)))(*[m._c for m in materials])
-        self._lights = (L.rb_area_light * max(1, len(area_lights)))(*[a._c for a in area_lights])
-        d.num_shapes, d.shapes = len(shapes), self._shapes
-        d.num_materials, d.materials = len(materials), self._materials
-        d.num_lights, d.lights = len(area_lights), self._lights
-        self._env = envmap._c if envmap is not None else None
-        d.envmap = C.pointer(self._env) if self._env is not None else None
-        d.use_gpu = int(bool(use_gpu))
-        d.gpu_index = int(gpu_index)
-        d.use_primary_edge_sampling = int(bool(use_primary_edge_sampling))
         if envmap is not None and use_secondary_edge_sampling:
             # The C ABI rejects this combination (the reference differentiates sky-side edge rays at stale hit points, DESIGN.md
             # section 7).  pyredner switches both edge samplers on by default, so an environment-lit scene arrives here with the flag
@@ -339,16 +326,12 @@ class Scene:  # src/redner.cpp:62-73, src/scene.cpp:63-307
             warnings.warn("redner_b200: secondary edge sampling is switched off for this scene (environment map, "
                           "RB_ENVMAP_WITHOUT_SECONDARY_EDGES=1); interior terms and primary edges are rendered and differentiated")
             use_secondary_edge_sampling = False
-        d.use_secondary_edge_sampling = int(bool(use_secondary_edge_sampling))
+        self.use_gpu = bool(use_gpu)
+        self.gpu_index = int(gpu_index)
+        self._flags = (int(bool(use_primary_edge_sampling)), int(bool(use_secondary_edge_sampling)))
+        d = self._desc(camera, shapes, materials, area_lights, envmap)
         h = C.c_void_p()
-        # build on the current PyTorch stream of the scene's device: the geometry tensors were produced there
-        stream = 0
-        try:
-            import torch
-            if use_gpu and torch.cuda.is_available():
-                stream = torch.cuda.current_stream(gpu_index if gpu_index >= 0 else None).cuda_stream
-        except ImportError:
-            pass
+        stream = self._stream()
         if hasattr(lib, "rb_scene_create_on_stream"):
             rc = lib.rb_scene_create_on_stream(C.byref(d), C.byref(h), C.c_void_p(stream or 0))
         else:
@@ -357,8 +340,32 @@ class Scene:  # src/redner.cpp:62-73, src/scene.cpp:63-307
             raise RuntimeError("redner.Scene: " + L.last_error(lib))
         self._handle = h
         self.max_generic_texture_dimension = lib.rb_scene_max_generic_texture_dimension(h)
-        self.use_gpu = bool(use_gpu)
-        self.gpu_index = int(gpu_index)
+
+    def _desc(self, camera, shapes, materials, area_lights, envmap):
+        d = L.rb_scene_desc()
+        d.camera = camera._c
+        self._shapes = (L.rb_shape * max(1, len(shapes)))(*[s._c for s in shapes])
+        self._materials = (L.rb_material * max(1, len(materials)))(*[m._c for m in materials])
+        self._lights = (L.rb_area_light * max(1, len(area_lights)))(*[a._c for a in area_lights])
+        d.num_shapes, d.shapes = len(shapes), self._shapes
+        d.num_materials, d.materials = len(materials), self._materials
+        d.num_lights, d.lights = len(area_lights), self._lights
+        self._env = envmap._c if envmap is not None else None
+        d.envmap = C.pointer(self._env) if self._env is not None else None
+        d.use_gpu = int(self.use_gpu)
+        d.gpu_index = self.gpu_index
+        d.use_primary_edge_sampling, d.use_secondary_edge_sampling = self._flags
+        return d
+
+    def _stream(self):
+        # the current PyTorch stream of the scene's device: the geometry tensors were produced there
+        try:
+            import torch
+            if self.use_gpu and torch.cuda.is_available():
+                return torch.cuda.current_stream(self.gpu_index if self.gpu_index >= 0 else None).cuda_stream
+        except ImportError:
+            pass
+        return 0
 
     # --- redner_b200 extensions (no reference counterpart) ---
     def set_partition(self, part, num_parts, rows_per_stripe=16):
@@ -369,6 +376,26 @@ class Scene:  # src/redner.cpp:62-73, src/scene.cpp:63-307
         """Re-target this scene at another camera; only the camera-dependent tables are rebuilt, on the device (rb_scene_set_camera)."""
         if self._lib.rb_scene_set_camera(self._handle, C.byref(camera._c)) != 0:
             raise RuntimeError("redner.Scene.set_camera: " + L.last_error(self._lib))
+
+    def update(self, camera, shapes, materials, area_lights, envmap, geometry_changed=True):
+        """Re-target this scene at shapes / materials / lights / environment map / camera of the SAME structure as its build, without
+        building a new scene (rb_scene_update): counts, ids and optional buffers as before, index buffers with the same contents.  Pass
+        geometry_changed=True when vertex positions may have been written in place; a new vertex buffer is noticed by itself."""
+        d = self._desc(camera, shapes, materials, area_lights, envmap)
+        if self._lib.rb_scene_update(self._handle, C.byref(d), int(bool(geometry_changed)), C.c_void_p(self._stream() or 0)) != 0:
+            raise RuntimeError("redner.Scene.update: " + L.last_error(self._lib))
+
+    def table(self, name):
+        """One table of the scene as the kernels see it, as raw bytes (rb_scene_table; names in _lib.RB_TABLES): test hook."""
+        import numpy as np
+        which = L.RB_TABLES.index(name)
+        n = C.c_size_t(0)
+        if self._lib.rb_scene_table(self._handle, which, None, 0, C.byref(n)) != 0:
+            raise RuntimeError("redner.Scene.table: " + L.last_error(self._lib))
+        out = np.zeros(n.value, dtype=np.uint8)
+        if n.value > 0 and self._lib.rb_scene_table(self._handle, which, out.ctypes.data_as(C.c_void_p), out.nbytes, C.byref(n)) != 0:
+            raise RuntimeError("redner.Scene.table: " + L.last_error(self._lib))
+        return out
 
     def last_stats(self):
         n = C.c_int(0)

@@ -29,6 +29,8 @@ struct rb_scene {
     std::vector<BVHTri> tris;
     std::vector<unsigned long long> sobol;
     int max_generic = 0;
+    int gpu_index = -1;
+    bool incomplete = false; // the last update failed part-way (as in the library: rb_render refuses the scene)
     int part = 0, num_parts = 1, rps = 16;
 };
 
@@ -71,20 +73,29 @@ static int build_node(rb_scene* sc, std::vector<int>& order, std::vector<float>&
     return me;
 }
 
-extern "C" int rb_scene_create(const rb_scene_desc* desc, rb_scene** out) {
-    if (const char* err = host_check_scene_desc(*desc)) {
-        g_err = err;
-        return 1;
-    }
-    rb_scene* sc = new rb_scene();
-    memset(&sc->dev, 0, sizeof(DevScene));
+static bool load_table(const char* path, size_t bytes_per, std::vector<unsigned char>& out, size_t count) {
+    FILE* f = fopen(path, "rb");
+    if (!f) return false;
+    out.resize(bytes_per * count);
+    bool ok = fread(out.data(), bytes_per, count, f) == count;
+    fclose(f);
+    return ok;
+}
+
+// Every table from the descriptor with the host builders (rb_scene_create and rb_scene_update).
+static int emu_build(rb_scene* sc, const rb_scene_desc* desc) {
+    DevScene& d = sc->dev;
+    const unsigned long long* sobol = d.sobol_matrices;
+    const float* ltc = d.ltc_table;
+    memset(&d, 0, sizeof(DevScene));
+    d.sobol_matrices = sobol;
+    d.sobol_dims = 1024;
     sc->cam = desc->camera;
-    host_setup_camera(desc->camera, sc->dev.cam);
+    host_setup_camera(desc->camera, d.cam);
     sc->shapes.assign(desc->shapes, desc->shapes + desc->num_shapes);
     sc->materials.assign(desc->materials, desc->materials + desc->num_materials);
     sc->lights = host_area_lights(*desc);
     sc->max_generic = host_max_generic_texture_dimension(*desc);
-    DevScene& d = sc->dev;
     d.edge_root_cs = d.edge_root_ncs = RB_EDGE_EMPTY;
     d.shapes = sc->shapes.data();
     d.num_shapes = (int)sc->shapes.size();
@@ -92,15 +103,9 @@ extern "C" int rb_scene_create(const rb_scene_desc* desc, rb_scene** out) {
     d.num_materials = (int)sc->materials.size();
     d.use_primary_edge = desc->use_primary_edge_sampling;
     d.use_secondary_edge = desc->use_secondary_edge_sampling;
-    // tables
-    FILE* f = fopen(RB_DATA_DIR "/sobol_joe_kuo_1024x52_u64.bin", "rb");
-    if (!f) { g_err = "emu: sobol table not found"; return 1; }
-    sc->sobol.resize(1024 * 52);
-    if (fread(sc->sobol.data(), 8, sc->sobol.size(), f) != sc->sobol.size()) { g_err = "emu: short sobol table"; return 1; }
-    fclose(f);
-    d.sobol_matrices = sc->sobol.data();
-    d.sobol_dims = 1024;
     // BVH
+    sc->nodes.clear();
+    sc->tris.clear();
     std::vector<float> boxes;
     for (int s = 0; s < d.num_shapes; s++)
         for (int t = 0; t < sc->shapes[s].num_triangles; t++) {
@@ -164,15 +169,74 @@ extern "C" int rb_scene_create(const rb_scene_desc* desc, rb_scene** out) {
             d.edge_root_cs = sc->tree.root_cs;
             d.edge_root_ncs = sc->tree.root_ncs;
             d.edge_bounds_expand = sc->tree.expand;
-            FILE* fl = fopen(RB_DATA_DIR "/ltc_blinn_phong_128x128x9_f32.bin", "rb");
-            if (!fl) { g_err = "emu: ltc table not found"; return 1; }
-            sc->ltc.resize(128 * 128 * 9);
-            if (fread(sc->ltc.data(), 4, sc->ltc.size(), fl) != sc->ltc.size()) { g_err = "emu: short ltc table"; return 1; }
-            fclose(fl);
-            d.ltc_table = sc->ltc.data();
+            d.ltc_table = ltc;
         }
     }
+    return 0;
+}
+
+extern "C" int rb_scene_create(const rb_scene_desc* desc, rb_scene** out) {
+    if (const char* err = host_check_scene_desc(*desc)) {
+        g_err = err;
+        return 1;
+    }
+    rb_scene* sc = new rb_scene();
+    memset(&sc->dev, 0, sizeof(DevScene));
+    sc->gpu_index = desc->gpu_index;
+    std::vector<unsigned char> bytes;
+    if (!load_table(RB_DATA_DIR "/sobol_joe_kuo_1024x52_u64.bin", 8, bytes, 1024 * 52)) { g_err = "emu: sobol table not found"; delete sc; return 1; }
+    sc->sobol.resize(1024 * 52);
+    memcpy(sc->sobol.data(), bytes.data(), bytes.size());
+    if (!load_table(RB_DATA_DIR "/ltc_blinn_phong_128x128x9_f32.bin", 4, bytes, 128 * 128 * 9)) { g_err = "emu: ltc table not found"; delete sc; return 1; }
+    sc->ltc.resize(128 * 128 * 9);
+    memcpy(sc->ltc.data(), bytes.data(), bytes.size());
+    sc->dev.sobol_matrices = sc->sobol.data();
+    sc->dev.ltc_table = sc->ltc.data();
+    if (emu_build(sc, desc)) {
+        delete sc;
+        return 1;
+    }
     *out = sc;
+    return 0;
+}
+// Re-target at a descriptor of the same structure: the same checks as the library, then every table is rebuilt from the descriptor with
+// the host builders (the library rebuilds only what changed, on the GPU; the tables are the same either way).
+extern "C" int rb_scene_update(rb_scene* sc, const rb_scene_desc* desc, int, void*) {
+    const char* err = host_check_scene_desc(*desc);
+    if (!err) err = host_check_same_structure(*desc, sc->shapes, (int)sc->materials.size(), sc->lights, sc->dev, sc->gpu_index, sc->max_generic);
+    if (err) {
+        g_err = err;
+        if (g_err.compare(0, 16, "rb_scene_create:") == 0) g_err = "rb_scene_update:" + g_err.substr(16);
+        return 1;
+    }
+    sc->incomplete = emu_build(sc, desc) != 0;
+    if (sc->incomplete && g_err.compare(0, 16, "rb_scene_create:") == 0) g_err = "rb_scene_update:" + g_err.substr(16);
+    return sc->incomplete ? 1 : 0;
+}
+extern "C" int rb_scene_table(const rb_scene* sc, int which, void* out, size_t bytes, size_t* size) {
+    const DevScene& d = sc->dev;
+    const bool prim = d.use_primary_edge && d.num_edges > 0, lights = d.num_lights > 0;
+    const void* src = nullptr;
+    size_t n = 0;
+    switch (which) {
+        case RB_TABLE_BVH_NODES: src = sc->nodes.data(); n = sizeof(BVHNode) * (size_t)std::max(d.num_tris - 1, 0); break;
+        case RB_TABLE_BVH_TRIANGLES: src = sc->tris.data(); n = sizeof(BVHTri) * sc->tris.size(); break;
+        case RB_TABLE_LIGHT_PMF: src = sc->lt.pmf.data(); n = lights ? sizeof(double) * sc->lt.pmf.size() : 0; break;
+        case RB_TABLE_LIGHT_CDF: src = sc->lt.cdf.data(); n = lights ? sizeof(double) * sc->lt.cdf.size() : 0; break;
+        case RB_TABLE_LIGHT_AREAS: src = sc->lt.areas.data(); n = lights ? sizeof(double) * sc->lt.areas.size() : 0; break;
+        case RB_TABLE_AREA_CDF_POOL: src = sc->lt.pool.data(); n = lights ? sizeof(double) * sc->lt.pool.size() : 0; break;
+        case RB_TABLE_AREA_CDF_OFFSETS: src = sc->lt.offsets.data(); n = lights ? sizeof(int) * sc->lt.offsets.size() : 0; break;
+        case RB_TABLE_PRIMARY_EDGE_PMF: src = sc->et.prim_pmf.data(); n = prim ? sizeof(double) * (size_t)d.num_edges : 0; break;
+        case RB_TABLE_PRIMARY_EDGE_CDF: src = sc->et.prim_cdf.data(); n = prim ? sizeof(double) * (size_t)d.num_edges : 0; break;
+        default: g_err = "rb_scene_table: unknown table"; return 1;
+    }
+    if (size) *size = n;
+    if (out && bytes > 0 && n > 0) memcpy(out, src, std::min(bytes, n));
+    return 0;
+}
+extern "C" int rb_scene_edge_list(const rb_scene* sc, int* num_edges, int* edges_out, size_t edges_bytes) {
+    if (num_edges) *num_edges = sc->dev.num_edges;
+    if (edges_out && edges_bytes > 0) memcpy(edges_out, sc->et.edges.data(), std::min(edges_bytes, sizeof(Edge) * (size_t)sc->dev.num_edges));
     return 0;
 }
 // Re-target at another camera: the camera-dependent tables (primary-edge distribution, both edge trees) are rebuilt with the host
@@ -226,6 +290,10 @@ extern "C" int rb_render(const rb_scene* scene, const rb_options* opt, float* im
                          float* screen_grad, void*) {
     if (!scene || !opt) {
         g_err = "rb_render: null scene / options";
+        return 1;
+    }
+    if (scene->incomplete) {
+        g_err = "rb_render: the scene's last update failed; update it again or build a new scene";
         return 1;
     }
     KernelArgs ka;
