@@ -275,6 +275,16 @@ enum rb_scene_table_id {
 };
 int rb_scene_table(const rb_scene* scene, int which, void* out, size_t bytes, size_t* size);
 
+/* Test hook: ray queries against the scene's triangle BVH.  All three buffers are memory of the scene's device.  rays: 8 floats per ray, { origin xyz,
+ * tnear, direction xyz, tfar }; ids receives { shape id, triangle id } per ray, { -1, -1 } for a miss; t the hit distance, tfar for a
+ * miss.  Without flags the query is the closest-hit traversal the render kernels call (rb_bvh.cuh, bvh_trace_impl), on the scene's own
+ * nodes, leaf triangles and root; RB_TRACE_ANY_HIT asks for its any-hit form.  RB_TRACE_BRUTE_FORCE skips the tree: the same triangle
+ * test on every leaf triangle in leaf order, with the traversal's early-outs (no triangles, |dir|^2 <= 1e-3, tfar < tnear); a closer hit
+ * replaces the best one only with a strictly smaller t, and an any-hit query stops at the first hit.  The exact answer the traversal
+ * must give.  Synchronises the device before and after. */
+enum rb_trace_flags { RB_TRACE_ANY_HIT = 1, RB_TRACE_BRUTE_FORCE = 2 };
+int rb_scene_trace_rays(const rb_scene* scene, const float* rays, int num_rays, int flags, int* ids, float* t);
+
 const char* rb_last_error(void);
 const char* rb_version(void);
 

@@ -19,6 +19,8 @@ c_int_p = C.POINTER(C.c_int)
 # enum rb_scene_table_id
 RB_TABLES = ("bvh_nodes", "bvh_triangles", "light_pmf", "light_cdf", "light_areas", "area_cdf_pool", "area_cdf_offsets", "primary_edge_pmf",
              "primary_edge_cdf")
+# enum rb_trace_flags
+RB_TRACE_ANY_HIT, RB_TRACE_BRUTE_FORCE = 1, 2
 
 
 class rb_camera(C.Structure):
@@ -114,7 +116,7 @@ class rb_dscene_desc(C.Structure):
 
 EXPORTS = [
     "rb_scene_create", "rb_scene_create_on_stream", "rb_scene_destroy", "rb_scene_max_generic_texture_dimension", "rb_compute_num_channels", "rb_render",
-    "rb_scene_set_partition", "rb_scene_last_stats", "rb_scene_last_stage_stats", "rb_scene_last_backward_stats", "rb_release_scratch", "rb_scene_build_ms", "rb_scene_edge_trees", "rb_scene_edge_list", "rb_scene_table", "rb_scene_set_camera", "rb_scene_update", "rb_render_batch", "rb_last_error", "rb_version",
+    "rb_scene_set_partition", "rb_scene_last_stats", "rb_scene_last_stage_stats", "rb_scene_last_backward_stats", "rb_release_scratch", "rb_scene_build_ms", "rb_scene_edge_trees", "rb_scene_edge_list", "rb_scene_table", "rb_scene_trace_rays", "rb_scene_set_camera", "rb_scene_update", "rb_render_batch", "rb_last_error", "rb_version",
 ]
 
 
@@ -166,6 +168,9 @@ def _bind(lib):
     if hasattr(lib, "rb_scene_table"):
         lib.rb_scene_table.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
         lib.rb_scene_table.restype = C.c_int
+    if hasattr(lib, "rb_scene_trace_rays"):
+        lib.rb_scene_trace_rays.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
+        lib.rb_scene_trace_rays.restype = C.c_int
     lib.rb_last_error.argtypes = []
     lib.rb_last_error.restype = C.c_char_p
     lib.rb_version.argtypes = []

@@ -141,6 +141,39 @@ RB_DFN BvhHit bvh_trace_impl(const float4* __restrict__ nodes4, const float4* __
     res.t = tfar;
     return res;
 }
+// The exact answer the traversal must give (test hook rb_scene_trace_rays): tri_test on every triangle in leaf order, with the
+// early-outs of bvh_trace_impl.  Closest hit: a triangle replaces the best hit only with a strictly smaller t, so of exactly tied
+// triangles the first in leaf order wins.  Any hit: the first triangle hit in leaf order.
+template <bool ANY_HIT>
+RB_D BvhHit bvh_brute_force(const float4* __restrict__ tris4, int num_tris, float ox, float oy, float oz, float dx, float dy, float dz,
+                            float tnear, float tfar) {
+    BvhHit res;
+    res.shape_id = -1;
+    res.tri_id = -1;
+    res.t = tfar;
+    res.hit = 0;
+    F3 O = f3(ox, oy, oz);
+    F3 D = f3(dx, dy, dz);
+    if (num_tris <= 0) return res;
+    if (D.x * D.x + D.y * D.y + D.z * D.z <= 1e-3f) return res;
+    if (!(tfar >= tnear)) return res;
+    for (int slot = 0; slot < num_tris; slot++) {
+        BVHTri tri;
+        tri.v0 = __ldg(tris4 + 3 * (size_t)slot + 0);
+        tri.v1 = __ldg(tris4 + 3 * (size_t)slot + 1);
+        tri.v2 = __ldg(tris4 + 3 * (size_t)slot + 2);
+        float t;
+        if (tri_test(O, D, tnear, tfar, tri, t) && (!res.hit || t < res.t)) {
+            res.hit = 1;
+            res.t = t;
+            res.shape_id = __float_as_int(tri.v0.w);
+            res.tri_id = __float_as_int(tri.v1.w);
+            if (ANY_HIT) break;
+        }
+    }
+    return res;
+}
+
 template <bool ANY_HIT>
 RB_D bool bvh_trace(const DevScene& sc, const Ray& ray, int& shape_id, int& tri_id, float& t_hit) {
     BvhHit h = bvh_trace_impl<ANY_HIT>(reinterpret_cast<const float4*>(sc.bvh_nodes), reinterpret_cast<const float4*>(sc.bvh_tris), sc.bvh_root,

@@ -11,6 +11,7 @@
 #include <type_traits>
 #include <vector>
 
+#include "rb_bvh.cuh"
 #include "rb_scene.cuh"
 #include "rb_scene_host.hpp"
 
@@ -678,6 +679,75 @@ extern "C" int rb_scene_table(const rb_scene* sc, int which, void* out, size_t b
             rb_set_error(std::string("rb_scene_table: ") + cudaGetErrorString(e));
             return 1;
         }
+    }
+    return 0;
+}
+
+// Test hook: one ray query per thread, through the traversal the render kernels call or by brute force over every triangle.
+template <bool ANY_HIT, bool BRUTE>
+__global__ void k_trace_rays(const float4* nodes4, const float4* tris4, int root, int num_tris, const float* rays, int num_rays, int* ids, float* t) {
+    int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= num_rays) return;
+    const float* r = rays + 8 * (size_t)i;
+    BvhHit h = BRUTE ? bvh_brute_force<ANY_HIT>(tris4, num_tris, r[0], r[1], r[2], r[4], r[5], r[6], r[3], r[7])
+                     : bvh_trace_impl<ANY_HIT>(nodes4, tris4, root, num_tris, r[0], r[1], r[2], r[4], r[5], r[6], r[3], r[7]);
+    ids[2 * (size_t)i] = h.shape_id;
+    ids[2 * (size_t)i + 1] = h.tri_id;
+    t[i] = h.t;
+}
+// (memory of the scene's own device: the kernel runs there, and another GPU's memory would be read without peer access)
+static bool on_device(const void* p, int device) {
+    cudaPointerAttributes a;
+    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
+        cudaGetLastError();
+        return false;
+    }
+    return (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) && a.device == device;
+}
+extern "C" int rb_scene_trace_rays(const rb_scene* sc, const float* rays, int num_rays, int flags, int* ids, float* t) {
+    if (!sc) {
+        rb_set_error("rb_scene_trace_rays: null scene");
+        return 1;
+    }
+    if (num_rays < 0) {
+        rb_set_error("rb_scene_trace_rays: negative number of rays");
+        return 1;
+    }
+    if (sc->incomplete) {
+        rb_set_error("rb_scene_trace_rays: the scene's last update failed; update it again or build a new scene");
+        return 1;
+    }
+    if (num_rays == 0) return 0;
+    int prev = 0;
+    cudaGetDevice(&prev);
+    if (cudaSetDevice(sc->device) != cudaSuccess) {
+        rb_set_error("rb_scene_trace_rays: cudaSetDevice failed");
+        return 1;
+    }
+    if (!on_device(rays, sc->device) || !on_device(ids, sc->device) || !on_device(t, sc->device)) {
+        cudaSetDevice(prev);
+        rb_set_error("rb_scene_trace_rays: rays, ids and t must be memory of the scene's device");
+        return 1;
+    }
+    // (synchronises the device before and after: the rays may come from any stream)
+    cudaError_t e = cudaDeviceSynchronize();
+    if (e == cudaSuccess) {
+        const float4* nodes4 = reinterpret_cast<const float4*>(sc->dev.bvh_nodes);
+        const float4* tris4 = reinterpret_cast<const float4*>(sc->dev.bvh_tris);
+        const int B = 128, G = (num_rays + B - 1) / B, root = sc->dev.bvh_root, T = sc->dev.num_tris;
+        switch (flags & (RB_TRACE_ANY_HIT | RB_TRACE_BRUTE_FORCE)) {
+            case 0: k_trace_rays<false, false><<<G, B>>>(nodes4, tris4, root, T, rays, num_rays, ids, t); break;
+            case RB_TRACE_ANY_HIT: k_trace_rays<true, false><<<G, B>>>(nodes4, tris4, root, T, rays, num_rays, ids, t); break;
+            case RB_TRACE_BRUTE_FORCE: k_trace_rays<false, true><<<G, B>>>(nodes4, tris4, root, T, rays, num_rays, ids, t); break;
+            default: k_trace_rays<true, true><<<G, B>>>(nodes4, tris4, root, T, rays, num_rays, ids, t); break;
+        }
+        e = cudaGetLastError();
+        if (e == cudaSuccess) e = cudaDeviceSynchronize();
+    }
+    cudaSetDevice(prev);
+    if (e != cudaSuccess) {
+        rb_set_error(std::string("rb_scene_trace_rays: ") + cudaGetErrorString(e));
+        return 1;
     }
     return 0;
 }

@@ -397,6 +397,22 @@ class Scene:  # src/redner.cpp:62-73, src/scene.cpp:63-307
             raise RuntimeError("redner.Scene.table: " + L.last_error(self._lib))
         return out
 
+    def trace_rays(self, rays, any_hit=False, brute_force=False):
+        """Ray queries against the scene's triangle BVH (rb_scene_trace_rays): test hook.  `rays` is an [N, 8] float32 tensor on the
+        scene's device (the outputs are allocated there too), rows (origin xyz, tnear, direction xyz, tfar).  Returns ([N, 2] int32 (shape id, triangle id), -1 for a miss;
+        [N] float32 hit distance, tfar for a miss).  `brute_force` tests every triangle instead of walking the tree."""
+        import torch
+        rays = rays.to(torch.float32).contiguous()
+        if rays.dim() != 2 or rays.shape[1] != 8:
+            raise ValueError("redner.Scene.trace_rays: rays must have shape [N, 8]")
+        n = rays.shape[0]
+        ids = torch.empty((n, 2), dtype=torch.int32, device=rays.device)
+        t = torch.empty(n, dtype=torch.float32, device=rays.device)
+        flags = (L.RB_TRACE_ANY_HIT if any_hit else 0) | (L.RB_TRACE_BRUTE_FORCE if brute_force else 0)
+        if self._lib.rb_scene_trace_rays(self._handle, C.c_void_p(rays.data_ptr()), n, flags, C.c_void_p(ids.data_ptr()), C.c_void_p(t.data_ptr())) != 0:
+            raise RuntimeError("redner.Scene.trace_rays: " + L.last_error(self._lib))
+        return ids, t
+
     def last_stats(self):
         n = C.c_int(0)
         ms = C.c_float(0)

@@ -1,6 +1,7 @@
 // DEVELOPMENT AID ONLY (see emu_shim.h).  Exports the same C ABI as libredner_b200.so, but every buffer is a HOST
 // pointer and the "kernels" are plain loops over the per-sample functions of rb_render.cuh.  The triangle BVH is a
-// simple median-split tree in the same node format (the GPU LBVH builder itself is exercised on the GPU only).
+// simple median-split tree in the same node format (the GPU LBVH builder itself is exercised on the GPU only, by
+// tests/test_bvh_gpu.py; rb_scene_trace_rays queries this tree with the same traversal).
 #include "emu_shim.h"
 
 #include <algorithm>
@@ -232,6 +233,30 @@ extern "C" int rb_scene_table(const rb_scene* sc, int which, void* out, size_t b
     }
     if (size) *size = n;
     if (out && bytes > 0 && n > 0) memcpy(out, src, std::min(bytes, n));
+    return 0;
+}
+// Ray queries against this build's median-split tree, through the same traversal and brute force as the library (host pointers).
+extern "C" int rb_scene_trace_rays(const rb_scene* sc, const float* rays, int num_rays, int flags, int* ids, float* t) {
+    if (!sc || num_rays < 0) {
+        g_err = !sc ? "rb_scene_trace_rays: null scene" : "rb_scene_trace_rays: negative number of rays";
+        return 1;
+    }
+    const DevScene& d = sc->dev;
+    const float4* nodes4 = reinterpret_cast<const float4*>(d.bvh_nodes);
+    const float4* tris4 = reinterpret_cast<const float4*>(d.bvh_tris);
+    for (int i = 0; i < num_rays; i++) {
+        const float* r = rays + 8 * (size_t)i;
+        BvhHit h;
+        switch (flags & (RB_TRACE_ANY_HIT | RB_TRACE_BRUTE_FORCE)) {
+            case 0: h = bvh_trace_impl<false>(nodes4, tris4, d.bvh_root, d.num_tris, r[0], r[1], r[2], r[4], r[5], r[6], r[3], r[7]); break;
+            case RB_TRACE_ANY_HIT: h = bvh_trace_impl<true>(nodes4, tris4, d.bvh_root, d.num_tris, r[0], r[1], r[2], r[4], r[5], r[6], r[3], r[7]); break;
+            case RB_TRACE_BRUTE_FORCE: h = bvh_brute_force<false>(tris4, d.num_tris, r[0], r[1], r[2], r[4], r[5], r[6], r[3], r[7]); break;
+            default: h = bvh_brute_force<true>(tris4, d.num_tris, r[0], r[1], r[2], r[4], r[5], r[6], r[3], r[7]); break;
+        }
+        ids[2 * (size_t)i] = h.shape_id;
+        ids[2 * (size_t)i + 1] = h.tri_id;
+        t[i] = h.t;
+    }
     return 0;
 }
 extern "C" int rb_scene_edge_list(const rb_scene* sc, int* num_edges, int* edges_out, size_t edges_bytes) {
