@@ -134,6 +134,13 @@ typedef struct rb_options {
     const int* channels; /* host array of rb_channel */
     int sampler_type;    /* rb_sampler_type */
     int sample_pixel_center;
+    /* 0: gradients are summed with float atomics, in whatever order the GPU schedules them (the last bits vary between runs).
+     * Non-zero: every gradient the backward pass writes -- every buffer of d_scene, the camera and screen_gradient_image -- is the
+     * correctly rounded exact sum of the per-sample float contributions, the same run after run whatever the band size, grid or
+     * device scheduling (fixed-point accumulators, DESIGN.md section 2).  It is added once into the caller's buffer; elements that
+     * received nothing are left as they are.  The accumulators take 88 bytes per gradient float from the backward scratch (see
+     * rb_release_scratch).  The forward pass is deterministic either way.  A zero-initialised struct keeps the default. */
+    int deterministic;
 } rb_options;
 
 /* DShape -- src/shape.h:65-80 (device pointers, any may be NULL) */
@@ -246,6 +253,10 @@ int rb_scene_last_stage_stats(const rb_scene* scene, float* stage_ms4, double* p
 /* Split of the backward bands of the last rb_render, summed over the bands:
  * { k_bwd_trace, scan + compaction + k_bwd_secondary, k_bwd_sweep } in milliseconds. */
 int rb_scene_last_backward_stats(const rb_scene* scene, float* bwd_ms3);
+/* Bytes of exact gradient accumulators (rb_options::deterministic) the last rb_render on this scene took from the backward scratch:
+ * 88 per accumulator, one per camera scalar and per float of the gradient buffers (overlapping buffers share them), plus a spare;
+ * 0 when the last call was not a deterministic backward pass. */
+int rb_scene_last_exact_bytes(const rb_scene* scene, size_t* bytes);
 /* rb_render keeps one grow-only scratch allocation per device for the backward pass (gradient descriptors, path
  * records, work lists; at most ~1 GiB + small).  This frees them all; the next backward pass allocates again. */
 void rb_release_scratch(void);
@@ -284,6 +295,12 @@ int rb_scene_table(const rb_scene* scene, int which, void* out, size_t bytes, si
  * must give.  Synchronises the device before and after. */
 enum rb_trace_flags { RB_TRACE_ANY_HIT = 1, RB_TRACE_BRUTE_FORCE = 2 };
 int rb_scene_trace_rays(const rb_scene* scene, const float* rays, int num_rays, int flags, int* ids, float* t);
+
+/* Test hook: exact sums through the scatter of the deterministic backward pass (warp aggregation and integer reductions included).
+ * values (float) and slots (int) are n device entries; contribution j of [0, n * repeat) adds values[j % n] to slot slots[j % n], so
+ * `repeat` drives slots past the per-accumulator bound between normalisations.  out_f32 / out_f64 (device, num_slots entries) receive
+ * each slot's sum rounded to float and to double (+0 for a slot without contributions).  Synchronises `stream`. */
+int rb_exact_sum_test(const float* values, const int* slots, int n, int num_slots, long long repeat, float* out_f32, double* out_f64, void* stream);
 
 const char* rb_last_error(void);
 const char* rb_version(void);

@@ -85,7 +85,7 @@ class rb_scene_desc(C.Structure):
 class rb_options(C.Structure):
     _fields_ = [
         ("seed", C.c_uint64), ("num_samples", C.c_int), ("max_bounces", C.c_int), ("num_channels", C.c_int),
-        ("channels", c_int_p), ("sampler_type", C.c_int), ("sample_pixel_center", C.c_int),
+        ("channels", c_int_p), ("sampler_type", C.c_int), ("sample_pixel_center", C.c_int), ("deterministic", C.c_int),
     ]
 
 
@@ -116,7 +116,7 @@ class rb_dscene_desc(C.Structure):
 
 EXPORTS = [
     "rb_scene_create", "rb_scene_create_on_stream", "rb_scene_destroy", "rb_scene_max_generic_texture_dimension", "rb_compute_num_channels", "rb_render",
-    "rb_scene_set_partition", "rb_scene_last_stats", "rb_scene_last_stage_stats", "rb_scene_last_backward_stats", "rb_release_scratch", "rb_scene_build_ms", "rb_scene_edge_trees", "rb_scene_edge_list", "rb_scene_table", "rb_scene_trace_rays", "rb_scene_set_camera", "rb_scene_update", "rb_render_batch", "rb_last_error", "rb_version",
+    "rb_scene_set_partition", "rb_scene_last_stats", "rb_scene_last_stage_stats", "rb_scene_last_backward_stats", "rb_scene_last_exact_bytes", "rb_release_scratch", "rb_scene_build_ms", "rb_scene_edge_trees", "rb_scene_edge_list", "rb_scene_table", "rb_scene_trace_rays", "rb_exact_sum_test", "rb_scene_set_camera", "rb_scene_update", "rb_render_batch", "rb_last_error", "rb_version",
 ]
 
 
@@ -149,6 +149,9 @@ def _bind(lib):
     if hasattr(lib, "rb_scene_last_backward_stats"):
         lib.rb_scene_last_backward_stats.argtypes = [C.c_void_p, c_float_p]
         lib.rb_scene_last_backward_stats.restype = C.c_int
+    if hasattr(lib, "rb_scene_last_exact_bytes"):
+        lib.rb_scene_last_exact_bytes.argtypes = [C.c_void_p, C.POINTER(C.c_size_t)]
+        lib.rb_scene_last_exact_bytes.restype = C.c_int
     if hasattr(lib, "rb_release_scratch"):
         lib.rb_release_scratch.argtypes = []
         lib.rb_release_scratch.restype = None
@@ -171,6 +174,9 @@ def _bind(lib):
     if hasattr(lib, "rb_scene_trace_rays"):
         lib.rb_scene_trace_rays.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
         lib.rb_scene_trace_rays.restype = C.c_int
+    if hasattr(lib, "rb_exact_sum_test"):
+        lib.rb_exact_sum_test.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_longlong, C.c_void_p, C.c_void_p, C.c_void_p]
+        lib.rb_exact_sum_test.restype = C.c_int
     lib.rb_last_error.argtypes = []
     lib.rb_last_error.restype = C.c_char_p
     lib.rb_version.argtypes = []

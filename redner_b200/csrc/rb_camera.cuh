@@ -10,6 +10,7 @@
 // (Brown-Conrady distortion is rejected by rb_scene_create).  A fisheye sample outside the unit disc gives a NULL ray
 // (zero origin and direction, src/camera.h:160-162): it is traced by nobody and contributes nothing.
 #pragma once
+#include "rb_atomic.cuh"
 #include "rb_types.cuh"
 
 struct D3 {
@@ -254,11 +255,26 @@ RB_HD M3 cam_m3(const double* a) {
 // column in shared memory; the block reduces once at kernel end and issues one double atomic per scalar.
 // Layout (RB_CAM_ACC floats): [0..15] d_cam_to_world, [16..31] d_world_to_cam, [32..40] d_intr_inv, [41..49] d_intr,
 // [50..57] d_distortion.
+// Deterministic mode (rb_kernels_det.cu) keeps one exact accumulator (rb_exact.cuh) per scalar for the whole block instead: each
+// (float) contribution goes there, the block flushes them into the global exact accumulators at kernel end.
 #define RB_CAM_ACC 58
 struct CamAcc {
+#if defined(RB_DETERMINISTIC) && !defined(RB_CPU_EMU)
+    long long* exact; // shared memory, [RB_CAM_ACC][RB_EXACT_WORDS]
+    RB_D void add(int k, Real v) { exact_agg_add(exact + k * RB_EXACT_WORDS, (float)v); }
+#else
     float* base; // shared memory, element k of this thread at base[k * stride]
     int stride;
+#ifdef RB_CPU_EMU
+    long long* exact = nullptr; // the emulator's deterministic mode: host exact accumulators, [RB_CAM_ACC][RB_EXACT_WORDS]
+    RB_D void add(int k, Real v) {
+        if (exact) exact_add_serial(exact + k * RB_EXACT_WORDS, (float)v);
+        else base[k * stride] += (float)v;
+    }
+#else
     RB_D void add(int k, Real v) { base[k * stride] += (float)v; }
+#endif
+#endif
     RB_D void add_c2w(const M4& d) {
         for (int i = 0; i < 4; i++)
             for (int j = 0; j < 4; j++)

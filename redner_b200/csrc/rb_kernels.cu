@@ -29,6 +29,7 @@
 #include "rb_kernel_set.h"
 #include "rb_render.cuh"
 #include "rb_scene.cuh"
+#include "rb_exact_layout.hpp"
 
 #include "rb_kernels_body.cuh"
 
@@ -121,6 +122,10 @@ extern "C" int rb_render(const rb_scene* scene_, const rb_options* opt, float* i
     const bool lean_allowed = getenv("RB_NO_LEAN") == nullptr; // (test hook: force the general kernels)
     const bool lean = lean_allowed && rp.only_radiance && !scene->dev.has_envmap && scene->dev.cam.type == RB_CAMERA_PERSPECTIVE && !scene->dev.cam.has_distortion;
     const RenderKernels kern = lean ? rb_lean::render_kernels() : render_kernels();
+    // Deterministic mode: the backward kernels of rb_kernels_det.cu (the forward kernels are deterministic as they are).
+    const bool det = opt->deterministic != 0;
+    const RenderKernels bkern = det ? rb_det::render_kernels() : kern;
+    const rb_det::ExactKernels xk = rb_det::exact_kernels();
 
     RenderGuard guard;
     int prev = 0;
@@ -139,6 +144,7 @@ extern "C" int rb_render(const rb_scene* scene_, const rb_options* opt, float* i
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, scene->device);
     std::vector<BandCounters> host_counters;
     long long num_bands_done = 0;
+    size_t exact_bytes = 0; // exact accumulators of a deterministic backward pass
     std::unique_lock<std::mutex> scratch_lock; // per-device scratch, held for the backward pass (released before the guard runs)
     void* args[] = {&scene->dev, &ka}; // parameters of every kernel in `kern` but the primary-edge pair (read at each launch)
     RB_CUDA_OK(cudaEventRecord(ev[EV_BEGIN], stream));
@@ -161,6 +167,19 @@ extern "C" int rb_render(const rb_scene* scene_, const rb_options* opt, float* i
             rb_set_error(err);
             return 1;
         }
+        ExactLayout xl;
+        if (det) {
+            exact_layout(*d_scene, scene->shapes.data(), scene->materials.data(), scene->dev, ka, xl);
+            ka.ds.env_values = xl.env_values;
+            ka.ds.env_w2e = xl.env_w2e;
+            ka.screen_grad = xl.screen_grad;
+        }
+        const size_t cam_smem_sweep = det ? RB_SMEM_CAM_EXACT : RB_SMEM_CAM(RB_BLOCK_SWEEP), cam_smem_prim = det ? RB_SMEM_CAM_EXACT : RB_SMEM_CAM(RB_BLOCK_PRIM);
+        const long long exact_max_samples = exact_band_samples(rp.max_bounces);
+        if (det && exact_max_samples < 1) {
+            rb_set_error("rb_render: deterministic mode supports at most 2097150 bounces");
+            return 1;
+        }
         const bool secondary = boundary_stage_runs(scene->dev, rp);
         const long long total_samples = (long long)ka.owned_rows * rp.vp_w * rp.spp;
         ka.rec_per_sample = rp.max_bounces + 1;
@@ -173,6 +192,7 @@ extern "C" int rb_render(const rb_scene* scene_, const rb_options* opt, float* i
         }
         long long band = (long long)std::max<size_t>(band_bytes / per_sample, 1024);
         band = std::min<long long>(band, (1LL << 30) / ka.rec_per_sample);
+        if (det) band = std::min(band, exact_max_samples);
         band = std::min<long long>(band, std::max<long long>(total_samples, 1));
         const long long num_bands = (total_samples + band - 1) / band;
         if (!events.ensure((size_t)(NUM_FIXED_EVENTS + BAND_EVENTS * num_bands))) {
@@ -188,7 +208,7 @@ extern "C" int rb_render(const rb_scene* scene_, const rb_options* opt, float* i
         const bool primary = primary_edge_pass_runs(scene->dev);
         const long long n_px_all = (long long)rp.vp_w * rp.vp_h;
         const long long total_e = primary ? ((n_px_all - rp.part + rp.num_parts - 1) / rp.num_parts) * rp.spp : 0; // i % num_parts == part
-        const long long band_e = std::min<long long>(std::max<long long>(total_e, 1), 1LL << 26);
+        const long long band_e = std::min<long long>(std::max<long long>(total_e, 1), det ? std::min(1LL << 26, exact_max_samples) : 1LL << 26);
         size_t sort_bytes = 0;
         cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, (const unsigned*)nullptr, (unsigned*)nullptr, (const unsigned*)nullptr, (unsigned*)nullptr, (int)band_e, 0, 32, stream);
 
@@ -202,6 +222,8 @@ extern "C" int rb_render(const rb_scene* scene_, const rb_options* opt, float* i
         double* cam_accum;
         BandCounters* counters;
         ListCount* list_offs;
+        long long* exact_acc; // deterministic mode: xl.num_acc accumulators and the spare
+        ExactRange* exact_ranges;
         void *scan_tmp, *sort_tmp;
         unsigned *k0, *k1, *v0, *v1;
         size_t zeroed_bytes = 0;
@@ -216,6 +238,8 @@ extern "C" int rb_render(const rb_scene* scene_, const rb_options* opt, float* i
             d_shapes = (rb_dshape*)take(std::max(1, d_scene->num_shapes) * sizeof(rb_dshape));
             d_mats = (rb_material*)take(std::max(1, d_scene->num_materials) * sizeof(rb_material));
             d_lights = (float**)take(std::max(1, d_scene->num_lights) * sizeof(float*));
+            exact_acc = (long long*)take(det ? (size_t)(xl.num_acc + 1) * RB_EXACT_WORDS * sizeof(long long) : 0);
+            exact_ranges = (ExactRange*)take(det ? std::max<size_t>(xl.ranges.size(), 1) * sizeof(ExactRange) : 0);
             // Every pass starts with these three at zero.  They stay adjacent, carved one after the other, so that one memset clears them.
             const size_t zeroed_begin = off;
             cam_accum = (double*)take(RB_CAM_ACC * sizeof(double));
@@ -252,15 +276,30 @@ extern "C" int rb_render(const rb_scene* scene_, const rb_options* opt, float* i
         scratch_lock = std::unique_lock<std::mutex>(dscratch.mutex);
         char* scratch = scratch_ensure(dscratch, scratch_bytes);
         if (!scratch) {
-            rb_set_error("rb_render: out of device memory for the backward scratch");
+            rb_set_error(det ? "rb_render: out of device memory for the backward scratch and the exact gradient accumulators of deterministic mode"
+                             : "rb_render: out of device memory for the backward scratch");
             return 1;
         }
         carve(scratch);
-        if (d_scene->num_shapes) RB_CUDA_OK(cudaMemcpyAsync(d_shapes, d_scene->shapes, d_scene->num_shapes * sizeof(rb_dshape), cudaMemcpyHostToDevice, stream));
+        // (deterministic mode: the descriptors with the virtual addresses of the accumulators; no kernel reads a gradient buffer)
+        const rb_dshape* h_shapes = det ? xl.shapes.data() : d_scene->shapes;
+        const rb_material* h_mats = det ? xl.materials.data() : d_scene->materials;
+        float* const* h_lights = det ? xl.lights.data() : d_scene->light_intensity;
+        if (d_scene->num_shapes) RB_CUDA_OK(cudaMemcpyAsync(d_shapes, h_shapes, d_scene->num_shapes * sizeof(rb_dshape), cudaMemcpyHostToDevice, stream));
         if (d_scene->num_materials)
-            RB_CUDA_OK(cudaMemcpyAsync(d_mats, d_scene->materials, d_scene->num_materials * sizeof(rb_material), cudaMemcpyHostToDevice, stream));
+            RB_CUDA_OK(cudaMemcpyAsync(d_mats, h_mats, d_scene->num_materials * sizeof(rb_material), cudaMemcpyHostToDevice, stream));
         if (d_scene->num_lights)
-            RB_CUDA_OK(cudaMemcpyAsync(d_lights, d_scene->light_intensity, d_scene->num_lights * sizeof(float*), cudaMemcpyHostToDevice, stream));
+            RB_CUDA_OK(cudaMemcpyAsync(d_lights, h_lights, d_scene->num_lights * sizeof(float*), cudaMemcpyHostToDevice, stream));
+        if (det) {
+            if (!xl.ranges.empty())
+                RB_CUDA_OK(cudaMemcpyAsync(exact_ranges, xl.ranges.data(), xl.ranges.size() * sizeof(ExactRange), cudaMemcpyHostToDevice, stream));
+            exact_bytes = (size_t)(xl.num_acc + 1) * RB_EXACT_WORDS * sizeof(long long);
+            RB_CUDA_OK(cudaMemsetAsync(exact_acc, 0, exact_bytes, stream));
+            RB_CUDA_OK((cudaError_t)rb_det::bind_exact_accumulators(exact_acc, stream));
+        }
+        long long n_acc = xl.num_acc;
+        void* normalise_args[] = {&exact_acc, &n_acc};
+        const int grid_x = sms * 4;
         RB_CUDA_OK(cudaMemsetAsync(cam_accum, 0, zeroed_bytes, stream)); // camera accumulators, band counters, edge histogram
         ka.ds.shapes = d_shapes;
         ka.ds.materials = d_mats;
@@ -269,10 +308,10 @@ extern "C" int rb_render(const rb_scene* scene_, const rb_options* opt, float* i
 
         // ---- interior + first-hit adjoints, band by band: trace (+ work lists) -> boundary terms (pick, counting sort by edge, shade)
         //      -> sweep.  Every list size stays on the device: fixed persistent grids, no host synchronisation inside the pass.
-        const int grid_t = pick_grid(kern.bwd_trace, scene->device, RB_BLOCK_TRACE);
-        const int grid_p = pick_grid(kern.bwd_sec_pick, scene->device, RB_BLOCK_SEC);
-        const int grid_s = pick_grid(kern.bwd_sec_shade, scene->device, RB_BLOCK_SEC);
-        const int grid_w = pick_grid(kern.bwd_sweep, scene->device, RB_BLOCK_SWEEP, RB_SMEM_CAM(RB_BLOCK_SWEEP));
+        const int grid_t = pick_grid(bkern.bwd_trace, scene->device, RB_BLOCK_TRACE);
+        const int grid_p = pick_grid(bkern.bwd_sec_pick, scene->device, RB_BLOCK_SEC);
+        const int grid_s = pick_grid(bkern.bwd_sec_shade, scene->device, RB_BLOCK_SEC);
+        const int grid_w = pick_grid(bkern.bwd_sweep, scene->device, RB_BLOCK_SWEEP, cam_smem_sweep);
         long long band_idx = 0;
         for (long long i0 = 0; i0 < total_samples; i0 += band, band_idx++) {
             ka.band_i0 = i0;
@@ -280,7 +319,7 @@ extern "C" int rb_render(const rb_scene* scene_, const rb_options* opt, float* i
             ka.counters = counters + band_idx;
             cudaEvent_t* bev = &ev[(size_t)(NUM_FIXED_EVENTS + BAND_EVENTS * band_idx)];
             RB_CUDA_OK(cudaEventRecord(bev[BAND_BEGIN], stream));
-            RB_CUDA_OK(cudaLaunchKernel(kern.bwd_trace, grid_t, RB_BLOCK_TRACE, args, 0, stream));
+            RB_CUDA_OK(cudaLaunchKernel(bkern.bwd_trace, grid_t, RB_BLOCK_TRACE, args, 0, stream));
             RB_CUDA_OK(cudaEventRecord(bev[BAND_AFTER_TRACE], stream));
             {
                 auto counts = thrust::make_transform_iterator(thrust::counting_iterator<int>(0), ListCountOf{ka.nrec, secondary ? ka.vmask : nullptr});
@@ -289,15 +328,19 @@ extern "C" int rb_render(const rb_scene* scene_, const rb_options* opt, float* i
             }
             launches += 4;
             if (secondary) {
-                RB_CUDA_OK(cudaLaunchKernel(kern.bwd_sec_pick, grid_p, RB_BLOCK_SEC, args, 0, stream));
+                RB_CUDA_OK(cudaLaunchKernel(bkern.bwd_sec_pick, grid_p, RB_BLOCK_SEC, args, 0, stream));
                 k_sec_offsets<<<1, 1024, 0, stream>>>(ka, scene->dev.num_edges);
                 k_sec_scatter<<<sms * 8, 256, 0, stream>>>(ka);
-                RB_CUDA_OK(cudaLaunchKernel(kern.bwd_sec_shade, grid_s, RB_BLOCK_SEC, args, 0, stream));
+                RB_CUDA_OK(cudaLaunchKernel(bkern.bwd_sec_shade, grid_s, RB_BLOCK_SEC, args, 0, stream));
                 launches += 4;
             }
             RB_CUDA_OK(cudaEventRecord(bev[BAND_BEFORE_SWEEP], stream));
-            RB_CUDA_OK(cudaLaunchKernel(kern.bwd_sweep, grid_w, RB_BLOCK_SWEEP, args, RB_SMEM_CAM(RB_BLOCK_SWEEP), stream));
+            RB_CUDA_OK(cudaLaunchKernel(bkern.bwd_sweep, grid_w, RB_BLOCK_SWEEP, args, cam_smem_sweep, stream));
             launches++;
+            if (det) {
+                RB_CUDA_OK(cudaLaunchKernel(xk.normalise, grid_x, 256, normalise_args, 0, stream));
+                launches++;
+            }
             RB_CUDA_OK(cudaEventRecord(bev[BAND_END], stream));
         }
         num_bands_done = band_idx;
@@ -307,7 +350,7 @@ extern "C" int rb_render(const rb_scene* scene_, const rb_options* opt, float* i
         }
         RB_CUDA_OK(cudaEventRecord(ev[EV_AFTER_BANDS], stream));
         if (primary) {
-            int grid_e = pick_grid(kern.primary_edge, scene->device, RB_BLOCK_PRIM, RB_SMEM_CAM(RB_BLOCK_PRIM));
+            int grid_e = pick_grid(bkern.primary_edge, scene->device, RB_BLOCK_PRIM, cam_smem_prim);
             int dim_base = primary_edge_dim_base(scene->dev, rp);
             int ebits = 1;
             while ((1 << ebits) < scene->dev.num_edges && ebits < 31) ebits++;
@@ -315,16 +358,26 @@ extern "C" int rb_render(const rb_scene* scene_, const rb_options* opt, float* i
                 int n = (int)std::min<long long>(band_e, total_e - t0);
                 int grid_k = std::min((n + 255) / 256, sms * 16);
                 void* key_args[] = {&scene->dev, &ka, &dim_base, &t0, &n, &k0, &v0};
-                RB_CUDA_OK(cudaLaunchKernel(kern.prim_keys, grid_k, 256, key_args, 0, stream));
+                RB_CUDA_OK(cudaLaunchKernel(bkern.prim_keys, grid_k, 256, key_args, 0, stream));
                 // sort on the edge bits and the top 8 bits of the position only (coarser order is enough for coherence)
                 int lo = std::max(0, 31 - ebits - 8);
                 cub::DeviceRadixSort::SortPairs(sort_tmp, sort_bytes, k0, k1, v0, v1, n, lo, 32, stream);
                 void* edge_args[] = {&scene->dev, &ka, &dim_base, &t0, &n, &k1, &v1};
-                RB_CUDA_OK(cudaLaunchKernel(kern.primary_edge, grid_e, RB_BLOCK_PRIM, edge_args, RB_SMEM_CAM(RB_BLOCK_PRIM), stream));
+                RB_CUDA_OK(cudaLaunchKernel(bkern.primary_edge, grid_e, RB_BLOCK_PRIM, edge_args, cam_smem_prim, stream));
                 launches += 2 + 4;
+                if (det) {
+                    RB_CUDA_OK(cudaLaunchKernel(xk.normalise, grid_x, 256, normalise_args, 0, stream));
+                    launches++;
+                }
             }
         }
         RB_CUDA_OK(cudaEventRecord(ev[EV_AFTER_PRIMARY_EDGE], stream));
+        if (det) { // round every accumulator once: into the caller's buffers, and the camera's into cam_accum
+            int num_ranges = (int)xl.ranges.size();
+            void* fin_args[] = {&exact_acc, &n_acc, &exact_ranges, &num_ranges, &cam_accum};
+            RB_CUDA_OK(cudaLaunchKernel(xk.finalise, grid_x, 256, fin_args, 0, stream));
+            launches++;
+        }
         k_finish_camera<<<1, 32, 0, stream>>>(scene->dev.cam, cam_accum, d_scene->camera);
         launches++;
         RB_CUDA_OK(cudaEventRecord(ev[EV_END], stream));
@@ -334,6 +387,7 @@ extern "C" int rb_render(const rb_scene* scene_, const rb_options* opt, float* i
     float ms = 0.f;
     cudaEventElapsedTime(&ms, ev[EV_BEGIN], ev[EV_END]);
     scene->last_launches = launches;
+    scene->last_exact_bytes = exact_bytes;
     scene->last_kernel_ms = ms;
     for (int i = EV_BEGIN; i < EV_END; i++) { // k_forward, backward bands, primary edges, k_finish_camera
         scene->last_stage_ms[i] = 0.f;
@@ -375,5 +429,53 @@ extern "C" int rb_render_batch(rb_scene* scene, int num_views, const rb_camera* 
         if (rb_scene_set_camera(scene, &cameras[k])) return 1;
         if (rb_render(scene, &options[k], images ? images[k] : nullptr, d_images ? d_images[k] : nullptr, d_scenes ? d_scenes[k] : nullptr, nullptr, stream)) return 1;
     }
+    return 0;
+}
+
+// Test hook: exact sums through the deterministic scatter (see the header).  Contribution j of [0, n * repeat) adds values[j % n] to
+// slot slots[j % n]; the slots are accumulators of the device scratch, normalised after every RB_EXACT_MAX_ADDS contributions.
+extern "C" int rb_exact_sum_test(const float* values, const int* slots, int n, int num_slots, long long repeat, float* out_f32, double* out_f64, void* stream_) {
+    if (n < 0 || num_slots < 0 || repeat < 0 || (n > 0 && (!values || !slots)) || (num_slots > 0 && (!out_f32 || !out_f64))) {
+        rb_set_error("rb_exact_sum_test: bad arguments");
+        return 1;
+    }
+    if (num_slots == 0) return 0;
+    cudaStream_t stream = (cudaStream_t)stream_;
+    std::vector<int> h_slots((size_t)n);
+    if (n > 0) { // (read on the caller's stream, which wrote them)
+        RB_CUDA_OK(cudaMemcpyAsync(h_slots.data(), slots, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost, stream));
+        RB_CUDA_OK(cudaStreamSynchronize(stream));
+    }
+    for (int s : h_slots)
+        if (s < 0 || s >= num_slots) {
+            rb_set_error("rb_exact_sum_test: slot out of range");
+            return 1;
+        }
+    int device = 0, sms = 132;
+    RB_CUDA_OK(cudaGetDevice(&device));
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
+    DeviceScratch& dscratch = g_scratch[device & 63];
+    std::lock_guard<std::mutex> lock(dscratch.mutex); // the accumulator binding is per device, like a backward pass
+    long long* acc = (long long*)scratch_ensure(dscratch, (size_t)num_slots * RB_EXACT_WORDS * sizeof(long long));
+    if (!acc) {
+        rb_set_error("rb_exact_sum_test: out of device memory");
+        return 1;
+    }
+    const rb_det::ExactKernels xk = rb_det::exact_kernels();
+    RB_CUDA_OK(cudaMemsetAsync(acc, 0, (size_t)num_slots * RB_EXACT_WORDS * sizeof(long long), stream));
+    RB_CUDA_OK((cudaError_t)rb_det::bind_exact_accumulators(acc, stream));
+    long long n_acc = num_slots;
+    void* normalise_args[] = {&acc, &n_acc};
+    const long long total = (long long)n * repeat;
+    for (long long j0 = 0; j0 < total; j0 += RB_EXACT_MAX_ADDS) {
+        long long count = std::min<long long>(RB_EXACT_MAX_ADDS, total - j0);
+        void* args[] = {(void*)&values, (void*)&slots, &n, &j0, &count};
+        RB_CUDA_OK(cudaLaunchKernel(xk.sum_test, sms * 8, 256, args, 0, stream));
+        RB_CUDA_OK(cudaLaunchKernel(xk.normalise, sms * 4, 256, normalise_args, 0, stream));
+    }
+    void* out_args[] = {&acc, &num_slots, &out_f32, &out_f64};
+    RB_CUDA_OK(cudaLaunchKernel(xk.readout, std::min((num_slots + 255) / 256, sms * 8), 256, out_args, 0, stream));
+    RB_CUDA_OK(cudaStreamSynchronize(stream));
+    RB_CUDA_OK(cudaGetLastError());
     return 0;
 }

@@ -14,6 +14,8 @@ constexpr int RB_BLOCK_SWEEP = 512, RB_MIN_BLOCKS_SWEEP = 1; // k_bwd_sweep
 constexpr int RB_BLOCK_PRIM = 128, RB_MIN_BLOCKS_PRIM = 5;   // k_primary_edge
 // dynamic shared memory: per-thread columns of the camera accumulators (k_bwd_sweep, k_primary_edge)
 #define RB_SMEM_CAM(block) ((size_t)RB_CAM_ACC * (block) * sizeof(float))
+// ... in the deterministic instantiation: the block's exact camera accumulators, [RB_CAM_ACC][RB_EXACT_WORDS]
+#define RB_SMEM_CAM_EXACT ((size_t)RB_CAM_ACC * RB_EXACT_WORDS * sizeof(long long))
 #ifndef RB_BAND_BYTES
 #define RB_BAND_BYTES (1ULL << 30) // scratch budget of one backward band (records + lists)
 #endif
@@ -170,6 +172,26 @@ RB_D void block_reduce_camera(float* cam_smem, double* cam_accum) {
         if (lane == 0 && s != 0.f) atomicAdd(&cam_accum[k], (double)s);
     }
 }
+#ifdef RB_DETERMINISTIC
+// Deterministic mode: the block's exact camera accumulators (shared memory, [RB_CAM_ACC][RB_EXACT_WORDS]) start at zero and end in
+// the global exact accumulators 0 .. RB_CAM_ACC - 1, normalised first so that a block adds less than 2^32 to each limb.
+RB_D void exact_camera_begin(long long* cam_exact) {
+    for (int i = threadIdx.x; i < RB_CAM_ACC * RB_EXACT_WORDS; i += blockDim.x) cam_exact[i] = 0;
+    __syncthreads();
+}
+RB_D void exact_camera_flush(long long* cam_exact) {
+    __syncthreads();
+    for (int k = threadIdx.x; k < RB_CAM_ACC; k += blockDim.x) {
+        long long a[RB_EXACT_WORDS];
+        for (int i = 0; i < RB_EXACT_WORDS; i++) a[i] = cam_exact[k * RB_EXACT_WORDS + i];
+        exact_normalise(a);
+        unsigned long long* g = (unsigned long long*)(rb_exact_acc + k * RB_EXACT_WORDS);
+        for (int i = 0; i < RB_EXACT_LIMBS; i++)
+            if (a[i] != 0) atomicAdd(g + i, (unsigned long long)a[i]);
+        if (a[RB_EXACT_LIMBS] != 0) atomicOr(g + RB_EXACT_LIMBS, (unsigned long long)a[RB_EXACT_LIMBS]);
+    }
+}
+#endif
 
 // Dense sample index of the band -> (pixel, px, py, s).  Consecutive lanes are consecutive samples of a pixel.
 struct SampleId {
@@ -401,11 +423,18 @@ __global__ void __launch_bounds__(RB_BLOCK_SEC, RB_MIN_BLOCKS_SEC) k_bwd_sec_sha
 }
 // Stage 3: reverse sweep of every path, first-hit and camera adjoints.
 __global__ void __launch_bounds__(RB_BLOCK_SWEEP, RB_MIN_BLOCKS_SWEEP) k_bwd_sweep(const __grid_constant__ DevScene sc, const __grid_constant__ KernelArgs ka) {
+#ifdef RB_DETERMINISTIC
+    extern __shared__ long long cam_exact[]; // [RB_CAM_ACC][RB_EXACT_WORDS]
+    exact_camera_begin(cam_exact);
+    CamAcc cam_acc;
+    cam_acc.exact = cam_exact;
+#else
     extern __shared__ float cam_smem[]; // [RB_CAM_ACC][blockDim.x]
     for (int k = 0; k < RB_CAM_ACC; k++) cam_smem[k * blockDim.x + threadIdx.x] = 0.f;
     CamAcc cam_acc;
     cam_acc.base = cam_smem + threadIdx.x;
     cam_acc.stride = blockDim.x;
+#endif
     const RenderParams& rp = ka.rp;
     const long long n = ka.counters->n_paths;
     RB_BLOCK_LOOP(t, n) {
@@ -415,7 +444,11 @@ __global__ void __launch_bounds__(RB_BLOCK_SWEEP, RB_MIN_BLOCKS_SWEEP) k_bwd_swe
         size_t base = (size_t)ts * ka.rec_per_sample;
         bwd_sweep(sc, ka, id.pixel, id.px, id.py, id.s, ka.records + base, 1, act ? ka.nrec[ts] : 0, ka.dpos ? ka.dpos + base : nullptr, cam_acc, act);
     }
+#ifdef RB_DETERMINISTIC
+    exact_camera_flush(cam_exact);
+#else
     block_reduce_camera(cam_smem, ka.ds.cam_accum);
+#endif
 }
 
 // ------------------------------------------------------------------------------------------------ primary edges
@@ -442,11 +475,18 @@ __global__ void __launch_bounds__(256) k_prim_keys(const __grid_constant__ DevSc
 }
 __global__ void __launch_bounds__(RB_BLOCK_PRIM, RB_MIN_BLOCKS_PRIM) k_primary_edge(const __grid_constant__ DevScene sc, const __grid_constant__ KernelArgs ka, int dim_base,
                                                                                long long t0, int n, const unsigned* keys, const unsigned* vals) {
+#ifdef RB_DETERMINISTIC
+    extern __shared__ long long cam_exact[]; // [RB_CAM_ACC][RB_EXACT_WORDS]
+    exact_camera_begin(cam_exact);
+    CamAcc cam_acc;
+    cam_acc.exact = cam_exact;
+#else
     extern __shared__ float cam_smem[]; // [RB_CAM_ACC][blockDim.x]
     for (int k = 0; k < RB_CAM_ACC; k++) cam_smem[k * blockDim.x + threadIdx.x] = 0.f;
     CamAcc cam_acc;
     cam_acc.base = cam_smem + threadIdx.x;
     cam_acc.stride = blockDim.x;
+#endif
     RB_BLOCK_LOOP(t, n) {
         RB_PRIM_SYNC();
         if (t < n && keys[t] != 0xffffffffu) {
@@ -456,7 +496,11 @@ __global__ void __launch_bounds__(RB_BLOCK_PRIM, RB_MIN_BLOCKS_PRIM) k_primary_e
             primary_edge_sample(sc, ka, i, s, dim_base, cam_acc);
         }
     }
+#ifdef RB_DETERMINISTIC
+    exact_camera_flush(cam_exact);
+#else
     block_reduce_camera(cam_smem, ka.ds.cam_accum);
+#endif
 }
 
 // The kernels of this instantiation that rb_render launches through a RenderKernels table (rb_kernel_set.h).

@@ -819,6 +819,11 @@ extern "C" int rb_scene_last_backward_stats(const rb_scene* sc, float* bwd_ms3) 
     for (int i = 0; i < 3; i++) bwd_ms3[i] = sc->last_bwd_ms[i];
     return 0;
 }
+extern "C" int rb_scene_last_exact_bytes(const rb_scene* sc, size_t* bytes) {
+    if (!sc || !bytes) return 1;
+    *bytes = sc->last_exact_bytes;
+    return 0;
+}
 extern "C" int rb_scene_build_ms(const rb_scene* sc, float* bvh_lights_edges3) {
     if (!sc || !bvh_lights_edges3) return 1;
     bvh_lights_edges3[0] = sc->build_ms_bvh;

@@ -59,6 +59,7 @@ struct rb_scene {
     float last_stage_ms[4] = {0.f, 0.f, 0.f, 0.f}; // k_forward, backward bands, k_primary_edge, k_finish_camera
     float last_bwd_ms[3] = {0.f, 0.f, 0.f};        // inside the bands: k_bwd_trace (+ work lists), boundary stage (pick, sort by edge, shade), k_bwd_sweep
     double last_path_vertices = 0, last_primary_hits = 0;
+    size_t last_exact_bytes = 0; // exact accumulators of the last deterministic backward pass (0 otherwise)
     int num_edge_nodes = 0; // records of the secondary-edge trees (dev.edge_nodes)
     bool edge_list_on_device = false;   // this scene's edge list was built by rb_edge_list.cu (else on the host)
     bool host_tables = false;           // ... and its camera-dependent tables on the host, from host_edges

@@ -419,6 +419,12 @@ class Scene:  # src/redner.cpp:62-73, src/scene.cpp:63-307
         self._lib.rb_scene_last_stats(self._handle, C.byref(n), C.byref(ms))
         return n.value, ms.value
 
+    def last_exact_bytes(self):
+        """Bytes of exact gradient accumulators the last render on this scene used (rb_scene_last_exact_bytes; 0 unless deterministic)."""
+        n = C.c_size_t(0)
+        self._lib.rb_scene_last_exact_bytes(self._handle, C.byref(n))
+        return n.value
+
     def last_stage_stats(self):
         """({kernel name: ms}, path_vertices, primary_hits) of the last render on this scene."""
         ms = (C.c_float * 4)()
@@ -485,7 +491,12 @@ class DScene:  # src/redner.cpp:75-82
 def render(scene, options, rendered_image, d_rendered_image, d_scene, screen_gradient_image, debug_image, stream=None):
     """src/redner.cpp:257 / src/pathtracer.cpp:177-183.  `debug_image` is accepted and ignored (the reference never
     reads it).  `stream` (a cudaStream_t value) is a redner_b200 extension; by default the current PyTorch stream is used
-    when torch is importable, else the legacy default stream."""
+    when torch is importable, else the legacy default stream.
+
+    Under `torch.use_deterministic_algorithms(True)` the backward pass runs in the library's deterministic mode
+    (rb_options.deterministic): every gradient is the correctly rounded exact sum of the per-sample contributions, bit for bit the
+    same from run to run, at some cost in time and 88 bytes of device scratch per gradient float.  There is no other switch; every
+    caller of this function (api.RenderFunction, api.SceneRenderer, api.render_batch, dist and the drop-in) follows PyTorch's."""
     lib = scene._lib
     o = L.rb_options()
     o.seed = options.seed
@@ -496,6 +507,11 @@ def render(scene, options, rendered_image, d_rendered_image, d_scene, screen_gra
     o.channels = chs
     o.sampler_type = options.sampler_type
     o.sample_pixel_center = int(options.sample_pixel_center)
+    try:
+        import torch
+        o.deterministic = int(torch.are_deterministic_algorithms_enabled())
+    except ImportError:
+        o.deterministic = 0
     if stream is None:
         try:
             import torch

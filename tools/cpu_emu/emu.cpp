@@ -10,6 +10,7 @@
 #include <vector>
 
 #include "../../redner_b200/csrc/rb_render.cuh"
+#include "../../redner_b200/csrc/rb_exact_layout.hpp"
 #include "../../redner_b200/csrc/rb_scene_host.hpp"
 
 static thread_local std::string g_err;
@@ -366,6 +367,31 @@ extern "C" int rb_render(const rb_scene* scene, const rb_options* opt, float* im
         CamAcc acc;
         acc.base = cam_f.data();
         acc.stride = 1;
+        // deterministic mode: every scatter and camera contribution into the exact accumulators of the library's layout
+        const bool det = opt->deterministic != 0;
+        ExactLayout xl;
+        std::vector<long long> xacc;
+        struct ExactReset {
+            ~ExactReset() { rb_emu_exact_acc = nullptr; }
+        } exact_reset;
+        long long exact_samples = 0;
+        const long long exact_max_samples = std::max(1LL, exact_band_samples(rp.max_bounces));
+        auto exact_sample_done = [&]() { // the library's bound: normalise after as many samples as one of its bands holds at most
+            if (det && ++exact_samples % exact_max_samples == 0)
+                for (long long i = 0; i <= xl.num_acc; i++) exact_normalise(&xacc[(size_t)i * RB_EXACT_WORDS]);
+        };
+        if (det) {
+            exact_layout(*d_scene, scene->shapes.data(), scene->materials.data(), sc, ka, xl);
+            xacc.assign((size_t)(xl.num_acc + 1) * RB_EXACT_WORDS, 0);
+            ka.ds.shapes = xl.shapes.data();
+            ka.ds.materials = xl.materials.data();
+            ka.ds.light_intensity = xl.lights.data();
+            ka.ds.env_values = xl.env_values;
+            ka.ds.env_w2e = xl.env_w2e;
+            ka.screen_grad = xl.screen_grad;
+            rb_emu_exact_acc = xacc.data();
+            acc.exact = xacc.data();
+        }
         std::vector<VertexRec> recs(rp.max_bounces + 2);
 #ifdef RB_EMU_REF_STREAMS
         // rank of every (sample, pixel) in the reference's compacted active list of each depth (pixels in ascending order)
@@ -389,6 +415,7 @@ extern "C" int rb_render(const rb_scene* scene, const rb_options* opt, float* im
 #endif
                     backward_sample(sc, ka, y * rp.vp_w + x, x, y, s, recs.data(), acc);
                     for (int k = 0; k < RB_CAM_ACC; k++) { cam_accum[k] += cam_f[k]; cam_f[k] = 0.f; }
+                    exact_sample_done();
                 }
         if (primary_edge_pass_runs(sc)) {
             long long n_px = (long long)rp.vp_w * rp.vp_h;
@@ -397,8 +424,11 @@ extern "C" int rb_render(const rb_scene* scene, const rb_options* opt, float* im
                     if (i % rp.num_parts != rp.part) continue; // primary-edge samples are sharded by sample index
                     primary_edge_sample(sc, ka, i, s, primary_edge_dim_base(sc, rp), acc);
                     for (int k = 0; k < RB_CAM_ACC; k++) { cam_accum[k] += cam_f[k]; cam_f[k] = 0.f; }
+                    exact_sample_done();
                 }
         }
+        if (det)
+            for (long long i = 0; i < xl.num_acc; i++) exact_finalise(xacc.data(), i, xl.ranges.data(), (int)xl.ranges.size(), cam_accum.data(), RB_CAM_ACC);
         finish_camera(sc.cam, cam_accum.data(), d_scene->camera);
     }
     return 0;
