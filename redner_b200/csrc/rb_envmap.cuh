@@ -36,9 +36,7 @@ RB_HD EnvUV envmap_uv(const DevEnvmap& e, V3 local_dir, const RayDiff& rd, bool 
 RB_HD V3 envmap_eval(const DevEnvmap& e, V3 dir, const RayDiff& rd) {
     V3 local_dir = normalize(env_xfm_vector(e.w2e, dir));
     EnvUV q = envmap_uv(e, local_dir, rd, local_dir.y < 1); // singular at (0, 1, 0): unfiltered there
-    Real o[3];
-    tex_eval(e.values, 3, q.uv, q.du_dxy, q.dv_dxy, o);
-    return mk3(o[0], o[1], o[2]);
+    return tex_eval(e.values, 3, q.uv, q.du_dxy, q.dv_dxy);
 }
 // d_values: gradient texture; d_w2e: 16 floats (row-major 4x4) accumulated with aggregated atomics
 RB_D void d_envmap_eval(const DevEnvmap& e, V3 dir, const RayDiff& rd, V3 d_out, const rb_texture& d_values, float* d_w2e, V3& d_dir, RayDiff& d_rd) {

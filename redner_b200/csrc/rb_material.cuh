@@ -38,8 +38,11 @@ RB_HD Real tex_level(const rb_texture& t, V2 du, V2 dv, Real& fu, Real& fv) {
     fv = length(dv) * t.height[0];
     return log2(rb_max(rb_max(fu, fv), Real(1e-8)));
 }
-// Mip-mapped (trilinear) fetch; out of line: ~15 inlined copies per kernel otherwise.  out[0..nch)
-RB_FN void tex_eval_mip(const rb_texture& t, int nch, V2 uv_, V2 du_dxy_, V2 dv_dxy_, Real* out) {
+// Mip-mapped (trilinear) fetch of channels c0, c0 + 1, c0 + 2 of an `nch`-channel texture; channels past nch - 1 repeat the last
+// one.  Out of line (~15 inlined copies per kernel otherwise) and returned by value, so that neither side keeps an addressable
+// array in local memory.
+RB_FN V3 tex_eval_mip(const rb_texture& t, int nch, int c0, V2 uv_, V2 du_dxy_, V2 dv_dxy_) {
+    const int c1 = c0 + 1 < nch ? c0 + 1 : nch - 1, c2 = c0 + 2 < nch ? c0 + 2 : nch - 1;
     Real sx = t.uv_scale[0], sy = t.uv_scale[1];
     V2 uv = mk2(uv_.x * sx, uv_.y * sy);
     V2 du = du_dxy_ * sx, dv = dv_dxy_ * sy;
@@ -48,23 +51,33 @@ RB_FN void tex_eval_mip(const rb_texture& t, int nch, V2 uv_, V2 du_dxy_, V2 dv_
     if (level <= 0 || level >= t.num_levels - 1) {
         int li = level <= 0 ? 0 : t.num_levels - 1;
         BilerpTap b = bilerp_tap(t, li, uv);
-        for (int c = 0; c < nch; c++) out[c] = bilerp_eval(t.texels[li], nch, c, b);
-    } else {
-        int li = (int)floor(level);
-        Real ld = level - li;
-        BilerpTap b0 = bilerp_tap(t, li, uv), b1 = bilerp_tap(t, li + 1, uv);
-        for (int c = 0; c < nch; c++) {
-            Real a0 = bilerp_eval(t.texels[li], nch, c, b0), a1 = bilerp_eval(t.texels[li + 1], nch, c, b1);
-            out[c] = a0 * (1 - ld) + a1 * ld;
-        }
+        const float* tex = t.texels[li];
+        return mk3(bilerp_eval(tex, nch, c0, b), bilerp_eval(tex, nch, c1, b), bilerp_eval(tex, nch, c2, b));
     }
+    int li = (int)floor(level);
+    Real ld = level - li;
+    BilerpTap b0 = bilerp_tap(t, li, uv), b1 = bilerp_tap(t, li + 1, uv);
+    const float *tex0 = t.texels[li], *tex1 = t.texels[li + 1];
+    V3 a0 = mk3(bilerp_eval(tex0, nch, c0, b0), bilerp_eval(tex0, nch, c1, b0), bilerp_eval(tex0, nch, c2, b0));
+    V3 a1 = mk3(bilerp_eval(tex1, nch, c0, b1), bilerp_eval(tex1, nch, c1, b1), bilerp_eval(tex1, nch, c2, b1));
+    return mk3(a0.x * (1 - ld) + a1.x * ld, a0.y * (1 - ld) + a1.y * ld, a0.z * (1 - ld) + a1.z * ld);
 }
-RB_HD void tex_eval(const rb_texture& t, int nch, V2 uv_, V2 du_dxy_, V2 dv_dxy_, Real* out) {
+// Channels c0 .. c0 + 2 of a texture lookup (see tex_eval_mip); a constant texture is read directly, without the call.
+RB_HD V3 tex_eval(const rb_texture& t, int nch, V2 uv_, V2 du_dxy_, V2 dv_dxy_, int c0 = 0) {
     if (tex_is_constant(t)) {
-        for (int c = 0; c < nch; c++) out[c] = t.texels[0][c];
-        return;
+        const float* v = t.texels[0];
+        return mk3(v[c0], v[c0 + 1 < nch ? c0 + 1 : nch - 1], v[c0 + 2 < nch ? c0 + 2 : nch - 1]);
     }
-    tex_eval_mip(t, nch, uv_, du_dxy_, dv_dxy_, out);
+    return tex_eval_mip(t, nch, c0, uv_, du_dxy_, dv_dxy_);
+}
+// All `nch` channels into out[0 .. nch) (textures of any width: the G-buffer's generic texture).
+RB_HD void tex_eval_channels(const rb_texture& t, int nch, V2 uv_, V2 du_dxy_, V2 dv_dxy_, Real* out) {
+    for (int c0 = 0; c0 < nch; c0 += 3) {
+        V3 v = tex_eval(t, nch, uv_, du_dxy_, dv_dxy_, c0);
+        out[c0] = v.x;
+        if (c0 + 1 < nch) out[c0 + 1] = v.y;
+        if (c0 + 2 < nch) out[c0 + 2] = v.z;
+    }
 }
 struct TexAdjoint { // returned by value so that the caller's SurfacePoint adjoint can stay in registers
     V2 d_uv, d_du_dxy, d_dv_dxy;
@@ -168,26 +181,10 @@ RB_D void d_tex_eval(const rb_texture& t, const rb_texture& d_t, int nch, V2 uv_
 }
 
 // ---------------------------------------------------------------- material helpers
-RB_HD V3 mat_diffuse(const rb_material& m, const SurfacePoint& p) {
-    Real o[3];
-    tex_eval(m.diffuse_reflectance, 3, p.uv, p.du_dxy, p.dv_dxy, o);
-    return mk3(o[0], o[1], o[2]);
-}
-RB_HD V3 mat_specular(const rb_material& m, const SurfacePoint& p) {
-    Real o[3];
-    tex_eval(m.specular_reflectance, 3, p.uv, p.du_dxy, p.dv_dxy, o);
-    return mk3(o[0], o[1], o[2]);
-}
-RB_HD Real mat_roughness(const rb_material& m, const SurfacePoint& p) {
-    Real o[1];
-    tex_eval(m.roughness, 1, p.uv, p.du_dxy, p.dv_dxy, o);
-    return o[0];
-}
-RB_HD V3 mat_normal_tex(const rb_material& m, const SurfacePoint& p) {
-    Real o[3];
-    tex_eval(m.normal_map, 3, p.uv, p.du_dxy, p.dv_dxy, o);
-    return mk3(o[0], o[1], o[2]);
-}
+RB_HD V3 mat_diffuse(const rb_material& m, const SurfacePoint& p) { return tex_eval(m.diffuse_reflectance, 3, p.uv, p.du_dxy, p.dv_dxy); }
+RB_HD V3 mat_specular(const rb_material& m, const SurfacePoint& p) { return tex_eval(m.specular_reflectance, 3, p.uv, p.du_dxy, p.dv_dxy); }
+RB_HD Real mat_roughness(const rb_material& m, const SurfacePoint& p) { return tex_eval(m.roughness, 1, p.uv, p.du_dxy, p.dv_dxy).x; }
+RB_HD V3 mat_normal_tex(const rb_material& m, const SurfacePoint& p) { return tex_eval(m.normal_map, 3, p.uv, p.du_dxy, p.dv_dxy); }
 RB_HD bool mat_has_normal_map(const rb_material& m) { return m.normal_map.num_levels > 0; }
 RB_HD Real roughness_to_phong(Real r) { return rb_max(2 / r - 2, Real(0)); }
 RB_HD Real d_roughness_to_phong(Real r, Real d_e) { return (r > 0 && r <= 1) ? -2 * d_e / rb_sq(r) : Real(0); }
@@ -222,6 +219,19 @@ RB_HD BsdfCtx bsdf_ctx(const rb_material& m, const SurfacePoint& p) {
     if (dot(c.geom_n, c.frame.n) < 0) c.geom_n = -c.geom_n;
     return c;
 }
+// The texture values the BSDF reads at one shading point.  trace_bounces fetches them once per vertex for its sample, eval and
+// pdf calls.  d_vertex goes through the overloads that fetch per call: holding the values across its body costs more spills there.
+struct MatTex {
+    V3 kd, ks;  // reflectances, clamped at zero
+    Real rough; // roughness as stored (each user clamps it its own way)
+};
+RB_HD MatTex mat_textures(const rb_material& m, const SurfacePoint& p) {
+    MatTex t;
+    t.kd = max3(m.use_vertex_color ? p.color : mat_diffuse(m, p), 0);
+    t.ks = max3(m.use_vertex_color ? zero3() : mat_specular(m, p), 0);
+    t.rough = mat_roughness(m, p);
+    return t;
+}
 RB_HD Real smith_g1(V3 v, V3 n, Real roughness) {
     Real cos_t = dot(v, n);
     Real tan_t = sqrt(rb_max(1 / (cos_t * cos_t) - 1, Real(0)));
@@ -233,16 +243,15 @@ RB_HD Real smith_g1(V3 v, V3 n, Real roughness) {
     return (Real(3.535) * a + Real(2.181) * a2) / (1 + Real(2.276) * a + Real(2.577) * a2);
 }
 
-RB_HD V3 bsdf_eval(const rb_material& m, const SurfacePoint& p, V3 wi, V3 wo, Real min_rough) {
+RB_HD V3 bsdf_eval(const rb_material& m, const SurfacePoint& p, const MatTex& tx, V3 wi, V3 wo, Real min_rough) {
     BsdfCtx c = bsdf_ctx(m, p);
     Real geom_wi = dot(c.geom_n, wi), geom_wo = dot(c.geom_n, wo);
     Real sh_wi = fabs(dot(c.frame.n, wi)), sh_wo = fabs(dot(c.frame.n, wo));
     if (geom_wi * geom_wo < 0) return zero3();
     if (!m.two_sided && geom_wi < 0 && geom_wo < 0) return zero3();
     if (sh_wi == 0 || sh_wo <= Real(1e-3) || fabs(geom_wo) <= Real(1e-3)) return zero3();
-    V3 kd = max3(m.use_vertex_color ? p.color : mat_diffuse(m, p), 0);
-    V3 ks = max3(m.use_vertex_color ? zero3() : mat_specular(m, p), 0);
-    Real roughness = rb_max(mat_roughness(m, p), min_rough);
+    const V3 kd = tx.kd, ks = tx.ks;
+    Real roughness = rb_max(tx.rough, min_rough);
     V3 diffuse = kd * (sh_wo / RB_PI);
     V3 spec = zero3();
     if (m.compute_specular_lighting && !m.use_vertex_color) {
@@ -260,16 +269,15 @@ RB_HD V3 bsdf_eval(const rb_material& m, const SurfacePoint& p, V3 wi, V3 wo, Re
     }
     return diffuse + spec;
 }
+RB_HD V3 bsdf_eval(const rb_material& m, const SurfacePoint& p, V3 wi, V3 wo, Real min_rough) { return bsdf_eval(m, p, mat_textures(m, p), wi, wo, min_rough); }
 
-RB_HD Real bsdf_pdf(const rb_material& m, const SurfacePoint& p, V3 wi, V3 wo, Real min_rough) {
+RB_HD Real bsdf_pdf(const rb_material& m, const SurfacePoint& p, const MatTex& tx, V3 wi, V3 wo, Real min_rough) {
     BsdfCtx c = bsdf_ctx(m, p);
     Real geom_wi = dot(c.geom_n, wi), geom_wo = dot(c.geom_n, wo);
     Real sh_wo = fabs(dot(c.frame.n, wo));
     if (geom_wi * geom_wo < 0) return 0;
     if (!m.two_sided && geom_wi < 0 && geom_wo < 0) return 0;
-    V3 kd = max3(m.use_vertex_color ? p.color : mat_diffuse(m, p), 0);
-    V3 ks = max3(m.use_vertex_color ? zero3() : mat_specular(m, p), 0);
-    Real wd = luminance(kd), ws = luminance(ks), wsum = wd + ws;
+    Real wd = luminance(tx.kd), ws = luminance(tx.ks), wsum = wd + ws;
     Real pd = Real(0.5), ps = Real(0.5);
     if (wsum > 0) {
         pd = wd / wsum;
@@ -285,7 +293,7 @@ RB_HD Real bsdf_pdf(const rb_material& m, const SurfacePoint& p, V3 wi, V3 wo, R
         if (m.two_sided && hl.z < 0) hl = -hl;
         Real hdwo = fabs(dot(h, wo));
         if (hl.z > 0 && hdwo > 0) {
-            Real roughness = rb_max(rb_max(mat_roughness(m, p), min_rough), Real(1e-6));
+            Real roughness = rb_max(rb_max(tx.rough, min_rough), Real(1e-6));
             Real e = roughness_to_phong(roughness);
             Real D = pow(hl.z, e) * (e + 2) / (2 * RB_PI);
             spec_pdf = ps * D * hl.z / (4 * hdwo);
@@ -293,18 +301,17 @@ RB_HD Real bsdf_pdf(const rb_material& m, const SurfacePoint& p, V3 wi, V3 wo, R
     }
     return diffuse_pdf + spec_pdf;
 }
+RB_HD Real bsdf_pdf(const rb_material& m, const SurfacePoint& p, V3 wi, V3 wo, Real min_rough) { return bsdf_pdf(m, p, mat_textures(m, p), wi, wo, min_rough); }
 
 // Returns the sampled direction (zero vector when sampling fails).  `w_sel` is the lobe-selection sample kept in
 // double so that the decision agrees with the reference's double comparison.
-RB_HD V3 bsdf_sample_dir(const rb_material& m, const SurfacePoint& p, V3 wi, V2 suv, double w_sel, Real min_rough, const RayDiff& wi_diff,
+RB_HD V3 bsdf_sample_dir(const rb_material& m, const SurfacePoint& p, const MatTex& tx, V3 wi, V2 suv, double w_sel, Real min_rough, const RayDiff& wi_diff,
                          RayDiff& wo_diff, Real& next_min_rough) {
     next_min_rough = min_rough;
     BsdfCtx c = bsdf_ctx(m, p);
     Real geom_wi = dot(c.geom_n, wi);
     if (!m.two_sided && geom_wi < 0) return zero3();
-    V3 kd = max3(m.use_vertex_color ? p.color : mat_diffuse(m, p), 0);
-    V3 ks = max3(m.use_vertex_color ? zero3() : mat_specular(m, p), 0);
-    Real wd = luminance(kd), ws = luminance(ks), wsum = wd + ws;
+    Real wd = luminance(tx.kd), ws = luminance(tx.ks), wsum = wd + ws;
     Real pd = Real(0.5);
     if (wsum > 0) pd = wd / wsum;
     if (w_sel <= (double)pd) {
@@ -320,7 +327,7 @@ RB_HD V3 bsdf_sample_dir(const rb_material& m, const SurfacePoint& p, V3 wi, V2 
         if (dot(c.geom_n, dir) * geom_wi < 0) dir = to_world(c.frame, -local);
         return dir;
     } else {
-        Real roughness = rb_max(rb_max(mat_roughness(m, p), min_rough), Real(1e-6));
+        Real roughness = rb_max(rb_max(tx.rough, min_rough), Real(1e-6));
         next_min_rough = rb_max(roughness, min_rough);
         Real e = roughness_to_phong(roughness);
         Real phi = 2 * RB_PI * suv.y;
@@ -348,8 +355,8 @@ RB_HD V3 bsdf_sample_dir(const rb_material& m, const SurfacePoint& p, V3 wi, V2 
 }
 
 // Adjoint of bsdf_eval with respect to material textures, the shading point, wi and wo.
-RB_D void d_bsdf_eval(const rb_material& m, const rb_material& d_m, const SurfacePoint& p, V3 wi, V3 wo, Real min_rough, V3 d_out,
-                      SurfacePoint& d_p, V3& d_wi, V3& d_wo) {
+RB_D void d_bsdf_eval(const rb_material& m, const rb_material& d_m, const SurfacePoint& p, const MatTex& tx, V3 wi, V3 wo, Real min_rough,
+                      V3 d_out, SurfacePoint& d_p, V3& d_wi, V3& d_wo) {
     BsdfCtx c = bsdf_ctx(m, p);
     const V3 n = c.frame.n;
     V3 d_n = zero3();
@@ -358,7 +365,7 @@ RB_D void d_bsdf_eval(const rb_material& m, const rb_material& d_m, const Surfac
     if (geom_wi * geom_wo < 0) return;
     if (!m.two_sided && geom_wi < 0 && geom_wo < 0) return;
     if (sh_wi == 0 || sh_wo <= Real(1e-3) || fabs(geom_wo) <= Real(1e-3)) return;
-    V3 kd = max3(m.use_vertex_color ? p.color : mat_diffuse(m, p), 0);
+    const V3 kd = tx.kd, ks = tx.ks;
     // diffuse = kd * sh_wo / pi   (gradient passes through the clamp unchanged, src/material.h:505-518)
     V3 d_kd = d_out * (sh_wo / RB_PI);
     if (m.use_vertex_color) d_p.color += d_kd;
@@ -370,8 +377,7 @@ RB_D void d_bsdf_eval(const rb_material& m, const rb_material& d_m, const Surfac
     d_wo += n * d_sh_wo;
     d_n += wo * d_sh_wo;
 
-    V3 ks = max3(m.use_vertex_color ? zero3() : mat_specular(m, p), 0);
-    Real roughness = rb_max(rb_max(mat_roughness(m, p), min_rough), Real(1e-6));
+    Real roughness = rb_max(rb_max(tx.rough, min_rough), Real(1e-6));
     if (m.compute_specular_lighting && !m.use_vertex_color) {
         V3 h = normalize(wi + wo);
         V3 hl = to_local(c.frame, h);
@@ -463,4 +469,8 @@ RB_D void d_bsdf_eval(const rb_material& m, const rb_material& d_m, const Surfac
         Real d_o[3] = {d.x, d.y, d.z};
         d_tex_eval(*t, *dt, k == 2 ? 1 : 3, p.uv, p.du_dxy, p.dv_dxy, d_o, d_p.uv, d_p.du_dxy, d_p.dv_dxy);
     }
+}
+RB_D void d_bsdf_eval(const rb_material& m, const rb_material& d_m, const SurfacePoint& p, V3 wi, V3 wo, Real min_rough, V3 d_out, SurfacePoint& d_p,
+                      V3& d_wi, V3& d_wo) {
+    d_bsdf_eval(m, d_m, p, mat_textures(m, p), wi, wo, min_rough, d_out, d_p, d_wi, d_wo);
 }

@@ -140,7 +140,7 @@ RB_D Real mis_power2(Real p_other, Real p_this) {
 
 // Radiance estimate at one vertex: returns nee + scatter (not yet multiplied by the throughput) and the
 // throughput factor for the next vertex.
-RB_D V3 vertex_estimate(const DevScene& sc, const rb_material& mat, const SurfacePoint& sp, V3 wi, Real min_rough, const LightSampleRec& ls,
+RB_D V3 vertex_estimate(const DevScene& sc, const rb_material& mat, const SurfacePoint& sp, const MatTex& tx, V3 wi, Real min_rough, const LightSampleRec& ls,
                         const SurfacePoint& lp, const Isect& bis, const SurfacePoint& bp, V3 bdir, V3& scatter_factor, bool& scatter_ok) {
     // Both estimators exist for two kinds of light (area light / environment map).  Each first settles the direction and
     // what the light contributes along it, then ONE bsdf_eval / bsdf_pdf pair serves either kind (the BSDF with its texture
@@ -173,8 +173,8 @@ RB_D V3 vertex_estimate(const DevScene& sc, const rb_material& mat, const Surfac
             }
         }
         if (on) {
-            V3 f = bsdf_eval(mat, sp, wi, wo, min_rough);
-            Real pdf_b = bsdf_pdf(mat, sp, wi, wo, min_rough) * G;
+            V3 f = bsdf_eval(mat, sp, tx, wi, wo, min_rough);
+            Real pdf_b = bsdf_pdf(mat, sp, tx, wi, wo, min_rough) * G;
             nee = (mis_power2(pdf_b, pdf_nee) * G / pdf_nee) * f * Le;
         }
     }
@@ -190,10 +190,10 @@ RB_D V3 vertex_estimate(const DevScene& sc, const rb_material& mat, const Surfac
             dist_sq = length_sq(dir);
             wo = dir / sqrt(dist_sq);
         }
-        Real pdf_b = bsdf_pdf(mat, sp, wi, wo, min_rough);
+        Real pdf_b = bsdf_pdf(mat, sp, tx, wi, wo, min_rough);
         // (hit: src/path_contribution.cpp:71-98; miss: :99-118 -- bdir is zero when the BSDF sample failed)
         if ((hit ? dist_sq > Real(1e-20) : length_sq(wo) > 0) && pdf_b > Real(1e-20)) {
-            V3 f = bsdf_eval(mat, sp, wi, wo, min_rough);
+            V3 f = bsdf_eval(mat, sp, tx, wi, wo, min_rough);
             if (hit) {
                 const rb_shape& bshape = sc.shapes[bis.shape_id];
                 if (bshape.light_id >= 0) {
@@ -262,7 +262,8 @@ RB_D V3 trace_bounces(const DevScene& sc, Sampler& smp, Ray ray, RayDiff rd_in, 
             }
             RayDiff rd_b;
             Real next_rough;
-            V3 dir = bsdf_sample_dir(mat, sp, wi, mk2((Real)bu, (Real)bv), bw, min_rough, rd, rd_b, next_rough);
+            const MatTex tx = mat_textures(mat, sp);
+            V3 dir = bsdf_sample_dir(mat, sp, tx, wi, mk2((Real)bu, (Real)bv), bw, min_rough, rd, rd_b, next_rough);
             Ray nray;
             nray.org = mk3((Real)p_d.x, (Real)p_d.y, (Real)p_d.z);
             nray.dir = dir;
@@ -276,7 +277,7 @@ RB_D V3 trace_bounces(const DevScene& sc, Sampler& smp, Ray ray, RayDiff rd_in, 
             if (closest_hit(sc, nray, bis)) bp = make_surface_point(sc.shapes[bis.shape_id], bis.tri_id, nray, rd_b, rd_after);
             V3 factor;
             bool ok;
-            V3 est = vertex_estimate(sc, mat, sp, wi, min_rough, ls, lp, bis, bp, dir, factor, ok);
+            V3 est = vertex_estimate(sc, mat, sp, tx, wi, min_rough, ls, lp, bis, bp, dir, factor, ok);
             L += thr * est;
             count++;
             thr = ok ? thr * factor : zero3();

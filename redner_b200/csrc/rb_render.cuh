@@ -260,7 +260,7 @@ RB_D void channel_values_at_hit(const DevScene& sc, const RenderParams& rp, cons
             case RB_CH_GENERIC_TEXTURE: {
                 if (mat.generic_texture.num_levels > 0) {
                     int n = mat.generic_texture.channels < RB_MAX_ND ? mat.generic_texture.channels : RB_MAX_ND;
-                    tex_eval(mat.generic_texture, n, sp.uv, sp.du_dxy, sp.dv_dxy, vals + d);
+                    tex_eval_channels(mat.generic_texture, n, sp.uv, sp.du_dxy, sp.dv_dxy, vals + d);
                 }
                 d += rp.max_generic;
             } break;
