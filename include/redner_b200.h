@@ -302,6 +302,16 @@ int rb_scene_trace_rays(const rb_scene* scene, const float* rays, int num_rays, 
  * each slot's sum rounded to float and to double (+0 for a slot without contributions).  Synchronises `stream`. */
 int rb_exact_sum_test(const float* values, const int* slots, int n, int num_slots, long long repeat, float* out_f32, double* out_f64, void* stream);
 
+/* Test hook: n texture lookups, one per thread, through the lookup and its adjoint that the render kernels call (rb_material.cuh).
+ * queries: [n, 6] floats per lookup { u, v, du/dx, du/dy, dv/dx, dv/dy }; values receives [n, channels].  1 and 3 channels take the
+ * BSDF's path (tex_eval from channel 0), other counts the generic texture's (tex_eval_channels).  With d_values ([n, channels]) the
+ * adjoint (d_tex_eval) scatters into d_tex -- same levels, sizes and channels as tex, zeroed by the caller, uv_scale may be NULL --
+ * and d_queries (may be NULL) receives { d_u, d_v, d(du/dx), d(du/dy), d(dv/dx), d(dv/dy) } per lookup.  Every buffer is memory of the
+ * current device; a negative n, channels < 1, num_levels outside [1, RB_MAX_MIP_LEVELS] or a level without a size (unless the
+ * texture is constant) are refused.  Runs on `stream` (a cudaStream_t, NULL == legacy default stream) and synchronises it. */
+int rb_texture_test(const rb_texture* tex, const rb_texture* d_tex, const float* queries, int n, const float* d_values, float* values,
+                    float* d_queries, void* stream);
+
 const char* rb_last_error(void);
 const char* rb_version(void);
 

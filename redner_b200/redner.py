@@ -473,6 +473,38 @@ class Scene:  # src/redner.cpp:62-73, src/scene.cpp:63-307
             pass
 
 
+def texture_test(tex, queries, d_values=None, d_tex=None):
+    """Texture lookups through the lookup and adjoint the render kernels call (rb_texture_test): test hook.  `tex` (and `d_tex`) are
+    Texture1 / Texture3 / TextureN; `queries` is an [N, 6] float32 tensor (u, v, du/dx, du/dy, dv/dx, dv/dy) on the textures' device,
+    which is made current.  Returns ([N, channels] values, [N, 6] d(queries) or None).  With `d_values` ([N, channels]) the adjoint
+    scatters into `d_tex`'s buffers (zeroed by the caller; its uv_scale may be NULL)."""
+    import torch
+    lib = L.load()
+    queries = queries.to(torch.float32).contiguous()
+    if queries.dim() != 2 or queries.shape[1] != 6:
+        raise ValueError("redner.texture_test: queries must have shape [N, 6]")
+    n, nch = queries.shape[0], int(tex._c.channels)
+    values = torch.empty((n, nch), dtype=torch.float32, device=queries.device)
+    d_queries = None
+    if d_values is not None:
+        d_values = d_values.to(torch.float32).contiguous()
+        if tuple(d_values.shape) != (n, nch):
+            raise ValueError("redner.texture_test: d_values must have shape [N, channels]")
+        if d_tex is None:
+            raise ValueError("redner.texture_test: d_values needs d_tex")
+        d_queries = torch.empty((n, 6), dtype=torch.float32, device=queries.device)
+    stream = 0
+    if queries.is_cuda:
+        torch.cuda.set_device(queries.device)
+        stream = torch.cuda.current_stream(queries.device).cuda_stream
+    ptr = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None  # noqa: E731
+    rc = lib.rb_texture_test(C.byref(tex._c), C.byref(d_tex._c) if d_tex is not None else None, ptr(queries), n, ptr(d_values), ptr(values),
+                             ptr(d_queries), C.c_void_p(stream or 0))
+    if rc != 0:
+        raise RuntimeError("redner.texture_test: " + L.last_error(lib))
+    return values, d_queries
+
+
 class DScene:  # src/redner.cpp:75-82
     def __init__(self, camera, shapes, materials, area_lights, envmap, use_gpu, gpu_index):
         d = L.rb_dscene_desc()

@@ -260,6 +260,55 @@ extern "C" int rb_scene_trace_rays(const rb_scene* sc, const float* rays, int nu
     }
     return 0;
 }
+// Texture lookups and adjoints through the same functions as the library's hook, one query after another (host pointers; the scatter
+// is the emulator's single-lane plain add).  The argument checks that do not involve device memory are the library's.
+extern "C" int rb_texture_test(const rb_texture* tex, const rb_texture* d_tex, const float* queries, int n, const float* d_values, float* values,
+                               float* d_queries, void*) {
+    const char* err = nullptr;
+    if (n < 0) err = "negative number of queries";
+    else if (tex == nullptr) err = "null texture";
+    else if (d_values != nullptr && d_tex == nullptr) err = "d_values needs a gradient texture";
+    else if (tex->channels < 1) err = "channels must be at least 1";
+    else if (tex->num_levels < 1 || tex->num_levels > RB_MAX_MIP_LEVELS) err = "num_levels must be in [1, RB_MAX_MIP_LEVELS]";
+    else if (d_values != nullptr && (d_tex->num_levels != tex->num_levels || d_tex->channels != tex->channels))
+        err = "the gradient texture must have the texture's levels and channels";
+    if (err == nullptr && !tex_is_constant(*tex))
+        for (int l = 0; l < tex->num_levels; l++)
+            if (tex->width[l] < 1 || tex->height[l] < 1) err = "every level of a texture that is not constant needs a positive width and height";
+    if (err != nullptr) {
+        g_err = std::string("rb_texture_test: ") + err;
+        return 1;
+    }
+    const int nch = tex->channels;
+    for (int i = 0; i < n; i++) {
+        const float* q = queries + 6 * (size_t)i;
+        const V2 uv = mk2(q[0], q[1]), du_dxy = mk2(q[2], q[3]), dv_dxy = mk2(q[4], q[5]);
+        float* out = values + (size_t)nch * i;
+        if (nch == 1 || nch == 3) {
+            const V3 v = tex_eval(*tex, nch, uv, du_dxy, dv_dxy);
+            out[0] = v.x;
+            if (nch == 3) {
+                out[1] = v.y;
+                out[2] = v.z;
+            }
+        } else {
+            tex_eval_channels(*tex, nch, uv, du_dxy, dv_dxy, out);
+        }
+        if (d_values == nullptr) continue;
+        V2 d_uv = zero2(), d_du = zero2(), d_dv = zero2();
+        d_tex_eval(*tex, *d_tex, nch, uv, du_dxy, dv_dxy, d_values + (size_t)nch * i, d_uv, d_du, d_dv);
+        if (d_queries != nullptr) {
+            float* dq = d_queries + 6 * (size_t)i;
+            dq[0] = d_uv.x;
+            dq[1] = d_uv.y;
+            dq[2] = d_du.x;
+            dq[3] = d_du.y;
+            dq[4] = d_dv.x;
+            dq[5] = d_dv.y;
+        }
+    }
+    return 0;
+}
 extern "C" int rb_scene_edge_list(const rb_scene* sc, int* num_edges, int* edges_out, size_t edges_bytes) {
     if (num_edges) *num_edges = sc->dev.num_edges;
     if (edges_out && edges_bytes > 0) memcpy(edges_out, sc->et.edges.data(), std::min(edges_bytes, sizeof(Edge) * (size_t)sc->dev.num_edges));
