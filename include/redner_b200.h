@@ -257,6 +257,29 @@ int rb_scene_last_backward_stats(const rb_scene* scene, float* bwd_ms3);
  * 88 per accumulator, one per camera scalar and per float of the gradient buffers (overlapping buffers share them), plus a spare;
  * 0 when the last call was not a deterministic backward pass. */
 int rb_scene_last_exact_bytes(const rb_scene* scene, size_t* bytes);
+/* Deterministic gradients summed over several calls, devices or processes (for example the stripes of rb_scene_set_partition on one
+ * GPU per rank).  Each call hands out its exact accumulators as RECORDS instead of rounding them; the caller sums the records, word by
+ * word in signed 64-bit integers (an all-reduce SUM), and rounds the sum once.  The gradients are then those of ONE deterministic
+ * rb_render over all the samples, bit for bit, however the samples were split.
+ * A record is 13 signed 64-bit words: 10 limbs of a fixed-point number (limb k weighs 2^(32 k - 149)) and three counts of non-finite
+ * contributions (+inf, -inf, NaN).  There are `count` records: one per camera gradient scalar, then one per float of every gradient
+ * buffer of d_scene and screen_gradient_image, in the order: shapes (vertices, uvs, normals, colors), materials (the five textures:
+ * levels, then uv_scale), light intensities, the environment map (levels, uv_scale, world_to_env), the screen-gradient image.  The
+ * position of a record depends on the structure of the descriptor only, never on where its buffers are; descriptors whose gradient
+ * buffers overlap are refused.  `fingerprint` hashes that structure: compare it across ranks before summing.  Records live in memory
+ * of the scene's device; `stream` as for rb_render, and both calls synchronise it. */
+int rb_exact_record_count(const rb_scene* scene, const rb_options* options, const rb_dscene_desc* d_scene, float* screen_gradient_image, size_t* count,
+                          uint64_t* fingerprint);
+/* The backward pass of rb_render in deterministic mode (whatever options->deterministic says), except its end: instead of rounding,
+ * every accumulator is ADDED into records[0, count) (zeroed by the caller, or holding the records of earlier calls), which are left
+ * normalised.  No buffer of d_scene or screen_gradient_image is written: their pointers only give the layout. */
+int rb_render_exact(const rb_scene* scene, const rb_options* options, const float* d_rendered_image, const rb_dscene_desc* d_scene,
+                    float* screen_gradient_image, long long* records, size_t count, void* stream);
+/* The end of a deterministic rb_render on records (any sum of records of this layout): every record that holds a non-zero value or a
+ * non-finite count is rounded once and added into the caller's gradient buffer, and the camera gradients are finished with the scene's
+ * camera.  Records that sum to zero leave their element untouched, as in rb_render. */
+int rb_exact_round(const rb_scene* scene, const rb_options* options, const rb_dscene_desc* d_scene, float* screen_gradient_image, const long long* records,
+                   size_t count, void* stream);
 /* rb_render keeps one grow-only scratch allocation per device for the backward pass (gradient descriptors, path
  * records, work lists; at most ~1 GiB + small).  This frees them all; the next backward pass allocates again. */
 void rb_release_scratch(void);

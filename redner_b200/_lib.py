@@ -21,6 +21,8 @@ RB_TABLES = ("bvh_nodes", "bvh_triangles", "light_pmf", "light_cdf", "light_area
              "primary_edge_cdf")
 # enum rb_trace_flags
 RB_TRACE_ANY_HIT, RB_TRACE_BRUTE_FORCE = 1, 2
+# int64 words per record of rb_render_exact / rb_exact_round: 10 limbs, then the counts of +inf, -inf and NaN contributions
+RB_EXACT_RECORD_WORDS = 13
 
 
 class rb_camera(C.Structure):
@@ -116,7 +118,7 @@ class rb_dscene_desc(C.Structure):
 
 EXPORTS = [
     "rb_scene_create", "rb_scene_create_on_stream", "rb_scene_destroy", "rb_scene_max_generic_texture_dimension", "rb_compute_num_channels", "rb_render",
-    "rb_scene_set_partition", "rb_scene_last_stats", "rb_scene_last_stage_stats", "rb_scene_last_backward_stats", "rb_scene_last_exact_bytes", "rb_release_scratch", "rb_scene_build_ms", "rb_scene_edge_trees", "rb_scene_edge_list", "rb_scene_table", "rb_scene_trace_rays", "rb_exact_sum_test", "rb_texture_test", "rb_scene_set_camera", "rb_scene_update", "rb_render_batch", "rb_last_error", "rb_version",
+    "rb_scene_set_partition", "rb_scene_last_stats", "rb_scene_last_stage_stats", "rb_scene_last_backward_stats", "rb_scene_last_exact_bytes", "rb_release_scratch", "rb_scene_build_ms", "rb_scene_edge_trees", "rb_scene_edge_list", "rb_scene_table", "rb_scene_trace_rays", "rb_exact_sum_test", "rb_texture_test", "rb_scene_set_camera", "rb_scene_update", "rb_render_batch", "rb_exact_record_count", "rb_render_exact", "rb_exact_round", "rb_last_error", "rb_version",
 ]
 
 
@@ -180,6 +182,15 @@ def _bind(lib):
     if hasattr(lib, "rb_texture_test"):
         lib.rb_texture_test.argtypes = [C.POINTER(rb_texture), C.POINTER(rb_texture), C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         lib.rb_texture_test.restype = C.c_int
+    if hasattr(lib, "rb_exact_record_count"):
+        lib.rb_exact_record_count.argtypes = [C.c_void_p, C.POINTER(rb_options), C.POINTER(rb_dscene_desc), C.c_void_p, C.POINTER(C.c_size_t),
+                                              C.POINTER(C.c_uint64)]
+        lib.rb_exact_record_count.restype = C.c_int
+        lib.rb_render_exact.argtypes = [C.c_void_p, C.POINTER(rb_options), C.c_void_p, C.POINTER(rb_dscene_desc), C.c_void_p, C.c_void_p, C.c_size_t,
+                                        C.c_void_p]
+        lib.rb_render_exact.restype = C.c_int
+        lib.rb_exact_round.argtypes = [C.c_void_p, C.POINTER(rb_options), C.POINTER(rb_dscene_desc), C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
+        lib.rb_exact_round.restype = C.c_int
     lib.rb_last_error.argtypes = []
     lib.rb_last_error.restype = C.c_char_p
     lib.rb_version.argtypes = []

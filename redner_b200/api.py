@@ -378,83 +378,102 @@ class RenderFunction(torch.autograd.Function):
         return img
 
     @staticmethod
-    def backward(ctx, grad_img):
-        c = ctx.c
+    def gradient_buffers(c, zeros=None):
+        """Zeroed gradient buffers for every differentiable input of the unpacked call `c`, and the DScene that points at them (`.d_scene`).
+        `zeros(*shape)` allocates one buffer (default: torch.zeros on c.device)."""
         rb, dev = c.backend, c.device
-        if not grad_img.is_contiguous():
-            grad_img = grad_img.contiguous()
-        assert torch.isfinite(grad_img).all()
-        z = lambda *shape: torch.zeros(*shape, device=dev)  # noqa: E731
+        z = zeros or (lambda *shape: torch.zeros(*shape, device=dev))
         fp = lambda t: _ptr(rb, t, "float")  # noqa: E731
+        g = _Ctx()
         if c.use_look_at:
             d_pos, d_look, d_up, d_c2w, d_w2c = z(3), z(3), z(3), None, None
         else:
             d_pos, d_look, d_up, d_c2w, d_w2c = None, None, None, z(4, 4), z(4, 4)
         d_intr_inv, d_intr = z(3, 3), z(3, 3)
         d_dist = z(8) if c.has_distortion else None
-        d_camera = rb.DCamera(fp(d_pos), fp(d_look), fp(d_up), fp(d_c2w), fp(d_w2c), fp(d_intr_inv), fp(d_intr), fp(d_dist))
-        d_shape_bufs, d_shapes = [], []
+        g.camera = (d_pos, d_look, d_up, d_c2w, d_w2c, d_intr_inv, d_intr, d_dist)
+        d_camera = rb.DCamera(*[fp(t) for t in g.camera])
+        g.shapes, d_shapes = [], []
         for v, i, uv, n, uvi, ni, col, mid, lid in c.shape_args:
             bufs = (z(*v.shape), z(*uv.shape) if uv is not None else None, z(*n.shape) if n is not None else None, z(*col.shape) if col is not None else None)
-            d_shape_bufs.append(bufs)
+            g.shapes.append(bufs)
             d_shapes.append(rb.DShape(fp(bufs[0]), fp(bufs[1]), fp(bufs[2]), fp(bufs[3])))
 
         def make_dtex(cls, t, nch_default):
             if t is None:
                 return None, cls([], [], [], nch_default, rb.float_ptr(0))
             mips, uv_scale = t
-            d_mips = [torch.zeros_like(m) for m in mips]
-            d_uv = torch.zeros(2, device=dev)
+            d_mips = [z(*m.shape) for m in mips]
+            d_uv = z(2)
             if mips[0].dim() == 3:
                 tex = cls([fp(m) for m in d_mips], [int(m.shape[1]) for m in mips], [int(m.shape[0]) for m in mips], int(mips[0].shape[2]), fp(d_uv))
             else:
                 tex = cls([fp(d_mips[0])], [0], [0], int(mips[0].shape[0]), fp(d_uv))
             return (d_mips, d_uv), tex
 
-        d_mat_bufs, d_materials = [], []
+        g.materials, d_materials = [], []
         for texs, spec, two_sided, vcol in c.mat_args:
             classes = (rb.Texture3, rb.Texture3, rb.Texture1, rb.TextureN, rb.Texture3)
             made = [make_dtex(cls, t, nd) for cls, t, nd in zip(classes, texs, (3, 3, 1, 0, 3))]
-            d_mat_bufs.append([m[0] for m in made])
+            g.materials.append([m[0] for m in made])
             d_materials.append(rb.DMaterial(*[m[1] for m in made]))
-        d_intensities = [z(3) for _ in c.light_args]
-        d_lights = [rb.DAreaLight(fp(t)) for t in d_intensities]
-        d_envmap, d_env_bufs = None, None
+        g.intensities = [z(3) for _ in c.light_args]
+        d_lights = [rb.DAreaLight(fp(t)) for t in g.intensities]
+        d_envmap, g.envmap = None, None
         if c.env_args is not None:  # pyredner/render_pytorch.py:948-968
             mips = c.env_args[0]
-            d_env_bufs = ([torch.zeros_like(m) for m in mips], torch.zeros(2, device=dev), torch.zeros(4, 4, device=dev))
-            d_env_tex = rb.Texture3([fp(m) for m in d_env_bufs[0]], [int(m.shape[1]) for m in mips], [int(m.shape[0]) for m in mips], 3, fp(d_env_bufs[1]))
-            d_envmap = rb.DEnvironmentMap(d_env_tex, fp(d_env_bufs[2]))
-        d_scene = rb.DScene(d_camera, d_shapes, d_materials, d_lights, d_envmap, dev.type == "cuda", dev.index if dev.index is not None else -1)
+            g.envmap = ([z(*m.shape) for m in mips], z(2), z(4, 4))
+            d_env_tex = rb.Texture3([fp(m) for m in g.envmap[0]], [int(m.shape[1]) for m in mips], [int(m.shape[0]) for m in mips], 3, fp(g.envmap[1]))
+            d_envmap = rb.DEnvironmentMap(d_env_tex, fp(g.envmap[2]))
+        g.d_scene = rb.DScene(d_camera, d_shapes, d_materials, d_lights, d_envmap, dev.type == "cuda", dev.index if dev.index is not None else -1)
+        return g
+
+    @staticmethod
+    def backward_options(c):
+        """The options of the backward pass of `c`: its second seed and sample count."""
         c.options.seed = c.seed[1]
         c.options.num_samples = c.num_samples[1]
-        screen_grad = getattr(c, "screen_gradient", None)  # (only set by visualize_screen_gradient)
-        rb.render(c.scene, c.options, rb.float_ptr(0), fp(grad_img), d_scene, fp(screen_grad), rb.float_ptr(0))
+        return c.options
 
+    @staticmethod
+    def gradient_outputs(c, g):
+        """backward's return value: the buffers of gradient_buffers(c) at the positions of serialize_scene's arguments."""
         out = [None]  # seed
         out += [None, None, None]  # counts
         cpu = lambda t: t.cpu() if t is not None else None  # noqa: E731
-        out += [cpu(d_pos), cpu(d_look), cpu(d_up), cpu(d_c2w), cpu(d_w2c), cpu(d_intr_inv), cpu(d_intr), cpu(d_dist)]
+        out += [cpu(t) for t in g.camera]
         out += [None, None, None, None]  # clip_near, resolution, viewport, camera_type
-        for bufs in d_shape_bufs:
+        for bufs in g.shapes:
             out += [bufs[0], None, bufs[1], bufs[2], None, None, bufs[3], None, None]
-        for mb, (texs, _, _, _) in zip(d_mat_bufs, c.mat_args):
+        for mb, (texs, _, _, _) in zip(g.materials, c.mat_args):
             for b, t in zip(mb, texs):
                 out.append(None)  # number of levels
                 if t is not None:
                     out += list(b[0])
                     out.append(b[1])
             out += [None, None, None]
-        for d_i in d_intensities:
+        for d_i in g.intensities:
             out += [None, d_i.cpu(), None, None]
-        if d_env_bufs is not None:  # pyredner/render_pytorch.py:1154-1164
+        if g.envmap is not None:  # pyredner/render_pytorch.py:1154-1164
             out.append(None)  # number of levels
-            out += list(d_env_bufs[0])
-            out += [d_env_bufs[1], None, d_env_bufs[2].cpu(), None, None, None, None]  # uv_scale, env_to_world, world_to_env, cdfs, pdf_norm, visible
+            out += list(g.envmap[0])
+            out += [g.envmap[1], None, g.envmap[2].cpu(), None, None, None, None]  # uv_scale, env_to_world, world_to_env, cdfs, pdf_norm, visible
         else:
             out.append(None)  # envmap
         out += [None] * 9  # num_samples .. backend
         return tuple(out)
+
+    @staticmethod
+    def backward(ctx, grad_img):
+        c = ctx.c
+        rb = c.backend
+        if not grad_img.is_contiguous():
+            grad_img = grad_img.contiguous()
+        assert torch.isfinite(grad_img).all()
+        g = RenderFunction.gradient_buffers(c)
+        screen_grad = getattr(c, "screen_gradient", None)  # (only set by visualize_screen_gradient)
+        rb.render(c.scene, RenderFunction.backward_options(c), rb.float_ptr(0), _ptr(rb, grad_img), g.d_scene, _ptr(rb, screen_grad), rb.float_ptr(0))
+        return RenderFunction.gradient_outputs(c, g)
 
 
 class BatchRenderFunction(torch.autograd.Function):

@@ -178,6 +178,16 @@ RB_HD double exact_to_double(const long long* acc) {
     const double v = ldexp((double)m, e - 149); // exact: m < 2^53 and the exponent stays inside the double range
     return neg ? -v : v;
 }
+// The range of accumulator i: the last of `ranges` (sorted by `first`) with first <= i.
+RB_HD int exact_range_of(long long i, const ExactRange* ranges, int num_ranges) {
+    int lo = 0, hi = num_ranges - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (ranges[mid].first <= i) lo = mid;
+        else hi = mid - 1;
+    }
+    return lo;
+}
 // Finalisation of accumulator i of a backward pass (the CUDA kernel k_exact_finalise and the host emulator): nothing if it received
 // nothing; the first `num_cam` accumulators are the camera scalars and become doubles in cam_accum; any other is rounded to float
 // and added once into the caller's element it stands for (`ranges` sorted by `first`).
@@ -188,11 +198,42 @@ RB_HD void exact_finalise(const long long* acc_all, long long i, const ExactRang
         cam_accum[i] = exact_to_double(a);
         return;
     }
-    int lo = 0, hi = num_ranges - 1; // last range with first <= i
-    while (lo < hi) {
-        const int mid = (lo + hi + 1) >> 1;
-        if (ranges[mid].first <= i) lo = mid;
-        else hi = mid - 1;
-    }
-    ranges[lo].dst[i - ranges[lo].first] += exact_to_float(a);
+    const int r = exact_range_of(i, ranges, num_ranges);
+    ranges[r].dst[i - ranges[r].first] += exact_to_float(a);
+}
+
+// Records: the form in which the accumulators of a backward pass leave one call (rb_render_exact) and come back to another
+// (rb_exact_round), possibly summed over calls, devices and processes in between.  One record is RB_EXACT_RECORD_WORDS signed 64-bit
+// words: the RB_EXACT_LIMBS limbs, then three COUNTS of non-finite contributions (+inf, -inf, NaN).  A sum of records, word by word, is
+// the record of the summed contributions: the limbs because integer addition is associative, the counts because a count stays
+// non-zero once set -- unlike the OR-ed flag bits of an accumulator, which a sum would turn into other bits (two +inf flags would add
+// up to the -inf flag).  Records are handed out normalised (exact_normalise), so N summed records have limbs below N * 2^32; an import
+// normalises again before anything looks at them.  Where a record sits depends on the structure of the gradient descriptor only
+// (ExactLayout::rec_first), not on where its buffers are.
+#define RB_EXACT_RECORD_WORDS (RB_EXACT_LIMBS + 3)
+// Record of accumulator i: the camera's first (record i), then rec_first[r] + (i - ranges[r].first) in range r.
+RB_HD long long exact_record_of(long long i, const ExactRange* ranges, const long long* rec_first, int num_ranges, int num_cam) {
+    if (i < num_cam) return i;
+    const int r = exact_range_of(i, ranges, num_ranges);
+    return rec_first[r] + (i - ranges[r].first);
+}
+// Adds accumulator `acc` into record `rec` and leaves the record normalised.
+RB_HD void exact_export(const long long* acc, long long* rec) {
+    long long a[RB_EXACT_LIMBS];
+    for (int k = 0; k < RB_EXACT_LIMBS; k++) a[k] = acc[k] + rec[k];
+    exact_normalise(a);
+    for (int k = 0; k < RB_EXACT_LIMBS; k++) rec[k] = a[k];
+    const long long f = acc[RB_EXACT_LIMBS];
+    rec[RB_EXACT_LIMBS] += (f & RB_EXACT_POS_INF) ? 1 : 0;
+    rec[RB_EXACT_LIMBS + 1] += (f & RB_EXACT_NEG_INF) ? 1 : 0;
+    rec[RB_EXACT_LIMBS + 2] += (f & RB_EXACT_NAN) ? 1 : 0;
+}
+// Accumulator `acc` from record `rec` (a sum of records, maybe): normalised limbs and the flag bits of the non-zero counts.  A record
+// whose value is zero and whose counts are zero gives an untouched accumulator, whatever its raw words were.
+RB_HD void exact_import(const long long* rec, long long* acc) {
+    long long a[RB_EXACT_LIMBS];
+    for (int k = 0; k < RB_EXACT_LIMBS; k++) a[k] = rec[k];
+    exact_normalise(a);
+    for (int k = 0; k < RB_EXACT_LIMBS; k++) acc[k] = a[k];
+    acc[RB_EXACT_LIMBS] = (rec[RB_EXACT_LIMBS] ? RB_EXACT_POS_INF : 0) | (rec[RB_EXACT_LIMBS + 1] ? RB_EXACT_NEG_INF : 0) | (rec[RB_EXACT_LIMBS + 2] ? RB_EXACT_NAN : 0);
 }

@@ -4,10 +4,19 @@
 // pointers are virtual addresses of those accumulators (rb_exact.cuh).  A NULL pointer stays NULL.  Caller buffers that overlap share
 // accumulators: the memory ranges are merged before they are numbered, so every caller float has exactly one accumulator and the
 // finalisation adds into it once.
+//
+// Accumulators are numbered in address order, which differs between processes and between descriptors of separately allocated
+// buffers.  Records (rb_exact.cuh), the form in which accumulators are summed across calls and devices, are numbered by the structure
+// of the descriptor alone: the camera scalars, then one record per float of every gradient buffer in the order exact_layout visits
+// them -- shapes (vertices, uvs, normals, colours), materials (the five textures: their levels, then uv_scale), light intensities, the
+// environment map (levels, uv_scale), world_to_env, the screen-gradient image.  Overlapping buffers have no such position: the entry
+// points that take or give records (rb_exact_record_count, rb_render_exact, rb_exact_round) refuse descriptors whose gradient buffers
+// overlap.  ExactLayout::fingerprint hashes that structure, so that callers can check that their records line up before they sum them.
 #pragma once
 #include <stdint.h>
 
 #include <algorithm>
+#include <string>
 #include <vector>
 
 #include "rb_exact.cuh"
@@ -26,6 +35,10 @@ inline long long exact_band_samples(int max_bounces) { return RB_EXACT_MAX_ADDS 
 struct ExactLayout {
     long long num_acc = 0;              // accumulators with a meaning; the array has one more, a spare (see virt below)
     std::vector<ExactRange> ranges;     // caller memory per accumulator range, sorted by `first`
+    std::vector<long long> rec_first;   // record of the first float of each range (meaningful when !overlaps)
+    long long num_records = 0;          // records: the camera scalars and every float of every span, in visiting order
+    bool overlaps = false;              // two gradient buffers overlap (and share accumulators)
+    uint64_t fingerprint = 0;           // FNV-1a of the structure: every buffer slot visited and its size (0 if absent)
     std::vector<rb_dshape> shapes;      // the descriptors with virtual addresses
     std::vector<rb_material> materials;
     std::vector<float*> lights;
@@ -41,10 +54,21 @@ inline void exact_layout(const rb_dscene_desc& d, const rb_shape* shapes, const 
                          ExactLayout& out) {
     struct Span {
         uintptr_t begin, end;
+        long long rec; // record of its first float
     };
     std::vector<Span> spans;
+    uint64_t h = 14695981039346656037ull;
+    auto hash = [&](uint64_t v) {
+        for (int b = 0; b < 8; b++) h = (h ^ ((v >> (8 * b)) & 0xffu)) * 1099511628211ull;
+    };
+    hash(RB_CAM_ACC);
+    out.num_records = RB_CAM_ACC;
     auto add = [&](const float* p, long long n) {
-        if (p != nullptr && n > 0) spans.push_back(Span{(uintptr_t)p, (uintptr_t)(p + n)});
+        const bool present = p != nullptr && n > 0;
+        hash(present ? (uint64_t)n : 0);
+        if (!present) return;
+        spans.push_back(Span{(uintptr_t)p, (uintptr_t)(p + n), out.num_records});
+        out.num_records += n;
     };
     // a texture's gradient: `nch` floats per texel (the channel count its d_tex_eval call uses), or per level of a constant texture
     auto add_texture = [&](const rb_texture& t, const rb_texture& dt, int nch) {
@@ -73,15 +97,20 @@ inline void exact_layout(const rb_dscene_desc& d, const rb_shape* shapes, const 
     if (sc.has_envmap) add_texture(sc.env.values, ka.ds.env_values, 3);
     add(ka.ds.env_w2e, 16);
     add(ka.screen_grad, 2LL * ka.rp.vp_w * ka.rp.vp_h);
+    hash((uint64_t)spans.size());
+    out.fingerprint = h;
 
     std::sort(spans.begin(), spans.end(), [](const Span& a, const Span& b) { return a.begin < b.begin; });
     out.ranges.clear();
+    out.rec_first.clear();
+    out.overlaps = false;
     out.num_acc = RB_CAM_ACC;
     for (const Span& sp : spans) {
         if (!out.ranges.empty()) {
             ExactRange& r = out.ranges.back();
             const uintptr_t end = (uintptr_t)(r.dst + r.count);
             if (sp.begin < end) { // overlaps the previous range: extend it
+                out.overlaps = true;
                 if (sp.end > end) {
                     const long long more = (long long)((sp.end - end) / sizeof(float));
                     r.count += more;
@@ -92,6 +121,7 @@ inline void exact_layout(const rb_dscene_desc& d, const rb_shape* shapes, const 
         }
         const long long n = (long long)((sp.end - sp.begin) / sizeof(float));
         out.ranges.push_back(ExactRange{out.num_acc, n, (float*)sp.begin});
+        out.rec_first.push_back(sp.rec);
         out.num_acc += n;
     }
     // caller pointer -> virtual address of its accumulator (NULL stays NULL).  A pointer of no range (a buffer of zero size) gets the
@@ -133,4 +163,20 @@ inline void exact_layout(const rb_dscene_desc& d, const rb_shape* shapes, const 
     out.env_values = virt_texture(ka.ds.env_values);
     out.env_w2e = virt(ka.ds.env_w2e);
     out.screen_grad = virt(ka.screen_grad);
+}
+
+// The records of a backward pass of `opt` over d_scene / screen_grad on a scene (camera `cam`, generic-texture width `max_generic`,
+// descriptors `shapes` / `materials`, device-side scene `sc`): the checks and the layout of rb_render's backward pass, and the refusal of
+// overlapping gradient buffers.  `who` prefixes the messages of this function's own checks.  Returns the error message, or null.
+inline const char* exact_record_layout(const char* who, const rb_options& opt, const rb_camera& cam, int max_generic, const rb_dscene_desc* d_scene,
+                                       float* screen_grad, const rb_shape* shapes, const rb_material* materials, const DevScene& sc, KernelArgs& ka,
+                                       ExactLayout& xl, std::string& err) {
+    if (d_scene == nullptr) return (err = std::string(who) + ": null d_scene").c_str();
+    static const float no_image = 0.f; // (the layout does not depend on the image: any non-null d_image passes the checks)
+    const char* e = setup_kernel_args(opt, cam, max_generic, 0, 1, 1, nullptr, &no_image, d_scene, screen_grad, ka);
+    if (e == nullptr) e = setup_backward(*d_scene, sc, ka);
+    if (e != nullptr) return e;
+    exact_layout(*d_scene, shapes, materials, sc, ka, xl);
+    if (xl.overlaps) return (err = std::string(who) + ": gradient buffers of d_scene overlap; records need disjoint buffers").c_str();
+    return nullptr;
 }

@@ -18,8 +18,10 @@ RenderKernels render_kernels();
 //   finalise   (const long long* acc, long long n, const ExactRange* ranges, int num_ranges, double* cam_accum)
 //   sum_test   (const float* values, const int* slots, int n, long long j0, long long count)
 //   readout    (const long long* acc, int n, float* out_f32, double* out_f64)
+//   export_records  (const long long* acc, long long n, const ExactRange* ranges, const long long* rec_first, int num_ranges, long long* records)
+//   import_records  (long long* acc, long long n, const ExactRange* ranges, const long long* rec_first, int num_ranges, const long long* records)
 struct ExactKernels {
-    const void *normalise, *finalise, *sum_test, *readout;
+    const void *normalise, *finalise, *sum_test, *readout, *export_records, *import_records;
 };
 ExactKernels exact_kernels();
 // Points the deterministic scatter at the accumulator array `acc` (stream-ordered); returns a cudaError_t.

@@ -98,8 +98,16 @@ static int pick_grid(const void* kernel, int device, int block = RB_BLOCK, size_
 enum { EV_BEGIN, EV_AFTER_FORWARD, EV_AFTER_BANDS, EV_AFTER_PRIMARY_EDGE, EV_END, NUM_FIXED_EVENTS };
 enum { BAND_BEGIN, BAND_AFTER_TRACE, BAND_BEFORE_SWEEP, BAND_END, BAND_EVENTS };
 
-extern "C" int rb_render(const rb_scene* scene_, const rb_options* opt, float* image, const float* d_image, const rb_dscene_desc* d_scene,
-                         float* screen_grad, void* stream_) {
+// The caller's records of rb_render_exact: the backward pass ends by adding its accumulators into them instead of rounding.
+struct ExactExport {
+    long long* records;
+    size_t count;
+};
+
+// rb_render and rb_render_exact: the same passes, which differ only in the last step of the backward pass (xo == nullptr: round into
+// the caller's buffers and finish the camera; otherwise: add the accumulators into xo->records).
+static int render_pass(const rb_scene* scene_, const rb_options* opt, float* image, const float* d_image, const rb_dscene_desc* d_scene,
+                       float* screen_grad, void* stream_, const ExactExport* xo) {
     rb_scene* scene = const_cast<rb_scene*>(scene_);
     if (!scene || !opt) {
         rb_set_error("rb_render: null scene / options");
@@ -122,8 +130,9 @@ extern "C" int rb_render(const rb_scene* scene_, const rb_options* opt, float* i
     const bool lean_allowed = getenv("RB_NO_LEAN") == nullptr; // (test hook: force the general kernels)
     const bool lean = lean_allowed && rp.only_radiance && !scene->dev.has_envmap && scene->dev.cam.type == RB_CAMERA_PERSPECTIVE && !scene->dev.cam.has_distortion;
     const RenderKernels kern = lean ? rb_lean::render_kernels() : render_kernels();
-    // Deterministic mode: the backward kernels of rb_kernels_det.cu (the forward kernels are deterministic as they are).
-    const bool det = opt->deterministic != 0;
+    // Deterministic mode: the backward kernels of rb_kernels_det.cu (the forward kernels are deterministic as they are).  Records
+    // come from the exact accumulators, so rb_render_exact runs them whatever the options say.
+    const bool det = opt->deterministic != 0 || xo != nullptr;
     const RenderKernels bkern = det ? rb_det::render_kernels() : kern;
     const rb_det::ExactKernels xk = rb_det::exact_kernels();
 
@@ -170,6 +179,15 @@ extern "C" int rb_render(const rb_scene* scene_, const rb_options* opt, float* i
         ExactLayout xl;
         if (det) {
             exact_layout(*d_scene, scene->shapes.data(), scene->materials.data(), scene->dev, ka, xl);
+            if (xo && xl.overlaps) {
+                rb_set_error("rb_render_exact: gradient buffers of d_scene overlap; records need disjoint buffers");
+                return 1;
+            }
+            if (xo && (size_t)xl.num_records != xo->count) {
+                rb_set_error("rb_render_exact: count is " + std::to_string(xo->count) + " but the descriptor has " + std::to_string(xl.num_records) +
+                             " records (rb_exact_record_count)");
+                return 1;
+            }
             ka.ds.env_values = xl.env_values;
             ka.ds.env_w2e = xl.env_w2e;
             ka.screen_grad = xl.screen_grad;
@@ -224,6 +242,7 @@ extern "C" int rb_render(const rb_scene* scene_, const rb_options* opt, float* i
         ListCount* list_offs;
         long long* exact_acc; // deterministic mode: xl.num_acc accumulators and the spare
         ExactRange* exact_ranges;
+        long long* exact_rec_first; // (rb_render_exact)
         void *scan_tmp, *sort_tmp;
         unsigned *k0, *k1, *v0, *v1;
         size_t zeroed_bytes = 0;
@@ -240,6 +259,7 @@ extern "C" int rb_render(const rb_scene* scene_, const rb_options* opt, float* i
             d_lights = (float**)take(std::max(1, d_scene->num_lights) * sizeof(float*));
             exact_acc = (long long*)take(det ? (size_t)(xl.num_acc + 1) * RB_EXACT_WORDS * sizeof(long long) : 0);
             exact_ranges = (ExactRange*)take(det ? std::max<size_t>(xl.ranges.size(), 1) * sizeof(ExactRange) : 0);
+            exact_rec_first = (long long*)take(xo ? std::max<size_t>(xl.rec_first.size(), 1) * sizeof(long long) : 0);
             // Every pass starts with these three at zero.  They stay adjacent, carved one after the other, so that one memset clears them.
             const size_t zeroed_begin = off;
             cam_accum = (double*)take(RB_CAM_ACC * sizeof(double));
@@ -293,6 +313,8 @@ extern "C" int rb_render(const rb_scene* scene_, const rb_options* opt, float* i
         if (det) {
             if (!xl.ranges.empty())
                 RB_CUDA_OK(cudaMemcpyAsync(exact_ranges, xl.ranges.data(), xl.ranges.size() * sizeof(ExactRange), cudaMemcpyHostToDevice, stream));
+            if (xo && !xl.rec_first.empty())
+                RB_CUDA_OK(cudaMemcpyAsync(exact_rec_first, xl.rec_first.data(), xl.rec_first.size() * sizeof(long long), cudaMemcpyHostToDevice, stream));
             exact_bytes = (size_t)(xl.num_acc + 1) * RB_EXACT_WORDS * sizeof(long long);
             RB_CUDA_OK(cudaMemsetAsync(exact_acc, 0, exact_bytes, stream));
             RB_CUDA_OK((cudaError_t)rb_det::bind_exact_accumulators(exact_acc, stream));
@@ -372,14 +394,21 @@ extern "C" int rb_render(const rb_scene* scene_, const rb_options* opt, float* i
             }
         }
         RB_CUDA_OK(cudaEventRecord(ev[EV_AFTER_PRIMARY_EDGE], stream));
-        if (det) { // round every accumulator once: into the caller's buffers, and the camera's into cam_accum
-            int num_ranges = (int)xl.ranges.size();
-            void* fin_args[] = {&exact_acc, &n_acc, &exact_ranges, &num_ranges, &cam_accum};
-            RB_CUDA_OK(cudaLaunchKernel(xk.finalise, grid_x, 256, fin_args, 0, stream));
+        int num_ranges = (int)xl.ranges.size();
+        if (xo) { // rb_render_exact: every accumulator, the camera's included, into the caller's records; no buffer of d_scene is written
+            long long* records = xo->records;
+            void* exp_args[] = {&exact_acc, &n_acc, &exact_ranges, &exact_rec_first, &num_ranges, &records};
+            RB_CUDA_OK(cudaLaunchKernel(xk.export_records, grid_x, 256, exp_args, 0, stream));
+            launches++;
+        } else {
+            if (det) { // round every accumulator once: into the caller's buffers, and the camera's into cam_accum
+                void* fin_args[] = {&exact_acc, &n_acc, &exact_ranges, &num_ranges, &cam_accum};
+                RB_CUDA_OK(cudaLaunchKernel(xk.finalise, grid_x, 256, fin_args, 0, stream));
+                launches++;
+            }
+            k_finish_camera<<<1, 32, 0, stream>>>(scene->dev.cam, cam_accum, d_scene->camera);
             launches++;
         }
-        k_finish_camera<<<1, 32, 0, stream>>>(scene->dev.cam, cam_accum, d_scene->camera);
-        launches++;
         RB_CUDA_OK(cudaEventRecord(ev[EV_END], stream));
     }
     cudaError_t err = cudaStreamSynchronize(stream);
@@ -412,6 +441,107 @@ extern "C" int rb_render(const rb_scene* scene_, const rb_options* opt, float* i
         rb_set_error(std::string("rb_render: kernel failure: ") + cudaGetErrorString(err));
         return 1;
     }
+    return 0;
+}
+
+extern "C" int rb_render(const rb_scene* scene, const rb_options* opt, float* image, const float* d_image, const rb_dscene_desc* d_scene,
+                         float* screen_grad, void* stream) {
+    return render_pass(scene, opt, image, d_image, d_scene, screen_grad, stream, nullptr);
+}
+
+// ------------------------------------------------------------------------------------------------ records (rb_exact.cuh)
+extern "C" int rb_exact_record_count(const rb_scene* scene, const rb_options* opt, const rb_dscene_desc* d_scene, float* screen_grad, size_t* count,
+                                     uint64_t* fingerprint) {
+    if (!scene || !opt || !count) {
+        rb_set_error("rb_exact_record_count: null scene / options / count");
+        return 1;
+    }
+    KernelArgs ka;
+    ExactLayout xl;
+    std::string err;
+    if (const char* e = exact_record_layout("rb_exact_record_count", *opt, scene->cam, scene->max_generic_texture_dimension, d_scene, screen_grad,
+                                            scene->shapes.data(), scene->materials.data(), scene->dev, ka, xl, err)) {
+        rb_set_error(e);
+        return 1;
+    }
+    *count = (size_t)xl.num_records;
+    if (fingerprint) *fingerprint = xl.fingerprint;
+    return 0;
+}
+
+extern "C" int rb_render_exact(const rb_scene* scene, const rb_options* opt, const float* d_image, const rb_dscene_desc* d_scene, float* screen_grad,
+                               long long* records, size_t count, void* stream) {
+    if (!d_image || !d_scene || !records) {
+        rb_set_error("rb_render_exact: null d_rendered_image / d_scene / records");
+        return 1;
+    }
+    const ExactExport xo{records, count};
+    return render_pass(scene, opt, nullptr, d_image, d_scene, screen_grad, stream, &xo);
+}
+
+extern "C" int rb_exact_round(const rb_scene* scene, const rb_options* opt, const rb_dscene_desc* d_scene, float* screen_grad, const long long* records,
+                              size_t count, void* stream_) {
+    if (!scene || !opt || !records) {
+        rb_set_error("rb_exact_round: null scene / options / records");
+        return 1;
+    }
+    if (scene->incomplete) {
+        rb_set_error("rb_exact_round: the scene's last update failed; update it again or build a new scene");
+        return 1;
+    }
+    KernelArgs ka;
+    ExactLayout xl;
+    std::string err;
+    if (const char* e = exact_record_layout("rb_exact_round", *opt, scene->cam, scene->max_generic_texture_dimension, d_scene, screen_grad, scene->shapes.data(),
+                                            scene->materials.data(), scene->dev, ka, xl, err)) {
+        rb_set_error(e);
+        return 1;
+    }
+    if ((size_t)xl.num_records != count) {
+        rb_set_error("rb_exact_round: count is " + std::to_string(count) + " but the descriptor has " + std::to_string(xl.num_records) +
+                     " records (rb_exact_record_count)");
+        return 1;
+    }
+    RenderGuard guard;
+    int prev = 0;
+    RB_CUDA_OK(cudaGetDevice(&prev));
+    RB_CUDA_OK(cudaSetDevice(scene->device));
+    guard.prev_device = prev;
+    cudaStream_t stream = (cudaStream_t)stream_;
+    int sms = 132;
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, scene->device);
+    // scratch: accumulators | ranges | record of each range | camera doubles, every buffer 256-byte aligned
+    auto align = [](size_t b) { return (b + 255) & ~(size_t)255; };
+    const size_t acc_bytes = align((size_t)(xl.num_acc + 1) * RB_EXACT_WORDS * sizeof(long long));
+    const size_t range_bytes = align(std::max<size_t>(xl.ranges.size(), 1) * sizeof(ExactRange));
+    const size_t rec_bytes = align(std::max<size_t>(xl.rec_first.size(), 1) * sizeof(long long));
+    DeviceScratch& dscratch = g_scratch[scene->device & 63];
+    std::lock_guard<std::mutex> lock(dscratch.mutex);
+    char* scratch = scratch_ensure(dscratch, acc_bytes + range_bytes + rec_bytes + RB_CAM_ACC * sizeof(double));
+    if (!scratch) {
+        rb_set_error("rb_exact_round: out of device memory for the exact accumulators");
+        return 1;
+    }
+    long long* acc = (long long*)scratch;
+    ExactRange* ranges = (ExactRange*)(scratch + acc_bytes);
+    long long* rec_first = (long long*)(scratch + acc_bytes + range_bytes);
+    double* cam_accum = (double*)(scratch + acc_bytes + range_bytes + rec_bytes);
+    if (!xl.ranges.empty()) {
+        RB_CUDA_OK(cudaMemcpyAsync(ranges, xl.ranges.data(), xl.ranges.size() * sizeof(ExactRange), cudaMemcpyHostToDevice, stream));
+        RB_CUDA_OK(cudaMemcpyAsync(rec_first, xl.rec_first.data(), xl.rec_first.size() * sizeof(long long), cudaMemcpyHostToDevice, stream));
+    }
+    RB_CUDA_OK(cudaMemsetAsync(cam_accum, 0, RB_CAM_ACC * sizeof(double), stream));
+    const rb_det::ExactKernels xk = rb_det::exact_kernels();
+    long long n_acc = xl.num_acc;
+    int num_ranges = (int)xl.ranges.size();
+    void* imp_args[] = {&acc, &n_acc, &ranges, &rec_first, &num_ranges, (void*)&records};
+    RB_CUDA_OK(cudaLaunchKernel(xk.import_records, sms * 4, 256, imp_args, 0, stream));
+    // from here on the end of a deterministic rb_render: round every accumulator once, then the camera
+    void* fin_args[] = {&acc, &n_acc, &ranges, &num_ranges, &cam_accum};
+    RB_CUDA_OK(cudaLaunchKernel(xk.finalise, sms * 4, 256, fin_args, 0, stream));
+    k_finish_camera<<<1, 32, 0, stream>>>(scene->dev.cam, cam_accum, d_scene->camera);
+    RB_CUDA_OK(cudaStreamSynchronize(stream));
+    RB_CUDA_OK(cudaGetLastError());
     return 0;
 }
 

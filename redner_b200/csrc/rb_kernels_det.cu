@@ -2,7 +2,8 @@
 // the general features, compiled with RB_DETERMINISTIC inside namespace rb_det.  Every gradient scatter then adds into exact
 // fixed-point accumulators (rb_exact.cuh, rb_atomic.cuh) instead of issuing float atomics, and the camera goes through exact
 // per-block accumulators, so the gradients do not depend on the order in which threads, warps and blocks add.  rb_render launches
-// these backward kernels when rb_options::deterministic is set, and the kernels below normalise, round and hand out the sums.
+// these backward kernels when rb_options::deterministic is set, rb_render_exact always, and the kernels below normalise, round and hand
+// out the sums, or move them to and from records.
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdint.h>
@@ -39,6 +40,17 @@ __global__ void k_exact_finalise(const long long* acc, long long n, const ExactR
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
         exact_finalise(acc, i, ranges, num_ranges, cam_accum, RB_CAM_ACC);
 }
+// rb_render_exact: every accumulator [0, n) is added into its record and the record left normalised (exact_export).  Accumulators
+// and records are disjoint one-to-one (the layout refuses overlapping buffers), so no two threads touch one record.
+__global__ void k_exact_export(const long long* acc, long long n, const ExactRange* ranges, const long long* rec_first, int num_ranges, long long* records) {
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+        exact_export(acc + i * RB_EXACT_WORDS, records + exact_record_of(i, ranges, rec_first, num_ranges, RB_CAM_ACC) * RB_EXACT_RECORD_WORDS);
+}
+// rb_exact_round: accumulators [0, n) from their records (exact_import), ready for k_exact_finalise.
+__global__ void k_exact_import(long long* acc, long long n, const ExactRange* ranges, const long long* rec_first, int num_ranges, const long long* records) {
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+        exact_import(records + exact_record_of(i, ranges, rec_first, num_ranges, RB_CAM_ACC) * RB_EXACT_RECORD_WORDS, acc + i * RB_EXACT_WORDS);
+}
 // Test hook rb_exact_sum_test: contribution j of [j0, j0 + count) adds values[j % n] to slot slots[j % n] through the scatter of the
 // render kernels (rb_red_add: the same warp aggregation and integer reductions), slot s being accumulator s.
 __global__ void k_exact_sum_test(const float* values, const int* slots, int n, long long j0, long long count) {
@@ -59,6 +71,8 @@ ExactKernels exact_kernels() {
     k.finalise = (const void*)k_exact_finalise;
     k.sum_test = (const void*)k_exact_sum_test;
     k.readout = (const void*)k_exact_readout;
+    k.export_records = (const void*)k_exact_export;
+    k.import_records = (const void*)k_exact_import;
     return k;
 }
 int bind_exact_accumulators(long long* acc, void* stream) {

@@ -6,7 +6,9 @@ Two ways to use N GPUs (SURVEY.md section 8e):
 * `render_tiles`  -- ONE image, split into round-robin stripes of viewport rows (rb_scene_set_partition).  Samplers stay
   seeded by the full-viewport pixel index, so the union over ranks equals the single-GPU image bit for bit; primary-edge
   samples are sharded by sample index.  One collective at the end of each pass: all_reduce(sum) of the framebuffer
-  (ranks hold zeros outside their stripes) after forward, and of the packed gradient buffers after backward.
+  (ranks hold zeros outside their stripes) after forward, and of the packed gradient buffers after backward.  Under
+  torch.use_deterministic_algorithms(True) the backward pass exchanges the exact accumulators instead (redner.render_exact, an integer
+  all_reduce, redner.round_exact), so every gradient is the one-GPU deterministic gradient bit for bit, for any number of ranks.
 * `render_poses` -- a batch of independent scenes / camera poses (BASELINE config 5): rank r renders poses r, r+N, ...;
   the only exchange is the all_reduce of the parameter gradients (the usual data-parallel multi-view optimisation).
 
@@ -48,6 +50,31 @@ def owned_rows(height: int, rank: int, world: int, rows_per_stripe: int = 4) -> 
     return [r for r in range(height) if (r // rows_per_stripe) % world == rank]
 
 
+def check_records_agree(count: int, fingerprint: int, device, group=None):
+    """Raises on every rank unless all ranks of `group` have the same record count and layout fingerprint (one all_gather)."""
+    mine = torch.tensor([count, fingerprint - (1 << 64) if fingerprint >= 1 << 63 else fingerprint], dtype=torch.int64, device=device)
+    every = [torch.empty_like(mine) for _ in range(dist.get_world_size(group))]
+    dist.all_gather(every, mine, group=group)
+    every = [tuple(int(v) for v in t.cpu()) for t in every]
+    if any(e != every[0] for e in every):
+        raise RuntimeError("redner_b200.dist: the ranks' gradient records do not line up (count, fingerprint per rank: %s); every rank must "
+                           "render the same scene structure" % every)
+
+
+def _exact_backward(c, grad_img, group):
+    """Deterministic backward pass of one sharded image: each rank's exact accumulators as records, one integer all_reduce, one rounding.
+    Integer sums do not depend on the order of the ranks or of NCCL's algorithm, so the gradients are the one-GPU deterministic ones."""
+    rb = c.backend
+    g = api.RenderFunction.gradient_buffers(c)
+    opts = api.RenderFunction.backward_options(c)
+    count, fingerprint = rb.exact_record_count(c.scene, opts, g.d_scene)
+    check_records_agree(count, fingerprint, c.device, group)
+    records = rb.render_exact(c.scene, opts, api._ptr(rb, grad_img.contiguous()), g.d_scene)
+    dist.all_reduce(records, op=dist.ReduceOp.SUM, group=group)
+    rb.round_exact(c.scene, opts, g.d_scene, None, records)  # (render_exact wrote none of g's buffers: they are still zero)
+    return api.RenderFunction.gradient_outputs(c, g)
+
+
 class TileRenderFunction(torch.autograd.Function):
     """RenderFunction for one image sharded over the ranks of a process group."""
 
@@ -70,6 +97,10 @@ class TileRenderFunction(torch.autograd.Function):
     @staticmethod
     def backward(ctx, grad_img):
         # every rank holds the full d_image (the loss is computed on the all-reduced image on every rank)
+        if torch.are_deterministic_algorithms_enabled():
+            grad_img = grad_img.contiguous()
+            assert torch.isfinite(grad_img).all()
+            return (None, None, None) + _exact_backward(ctx.c, grad_img, ctx.group)[1:]
         ctx_like = type("C", (), {})()
         ctx_like.c, ctx_like.args = ctx.c, ctx.args
         grads = api.RenderFunction.backward(ctx_like, grad_img)

@@ -520,6 +520,38 @@ class DScene:  # src/redner.cpp:75-82
         self._c = d
 
 
+def _options(options, deterministic=None):
+    """rb_options of a RenderOptions; the channel array is kept alive by the returned tuple."""
+    o = L.rb_options()
+    o.seed = options.seed
+    o.num_samples = options.num_samples
+    o.max_bounces = options.max_bounces
+    chs = (C.c_int * max(1, len(options.channels)))(*options.channels)
+    o.num_channels = len(options.channels)
+    o.channels = chs
+    o.sampler_type = options.sampler_type
+    o.sample_pixel_center = int(options.sample_pixel_center)
+    if deterministic is None:
+        try:
+            import torch
+            deterministic = torch.are_deterministic_algorithms_enabled()
+        except ImportError:
+            deterministic = False
+    o.deterministic = int(bool(deterministic))
+    return o, chs
+
+
+def _render_stream(scene, stream):
+    if stream is None:
+        try:
+            import torch
+            # (the stream of the SCENE's device: a stream handle of another device would be invalid there)
+            stream = torch.cuda.current_stream(scene.gpu_index if scene.gpu_index >= 0 else None).cuda_stream if torch.cuda.is_available() else 0
+        except Exception:
+            stream = 0
+    return C.c_void_p(stream or 0)
+
+
 def render(scene, options, rendered_image, d_rendered_image, d_scene, screen_gradient_image, debug_image, stream=None):
     """src/redner.cpp:257 / src/pathtracer.cpp:177-183.  `debug_image` is accepted and ignored (the reference never
     reads it).  `stream` (a cudaStream_t value) is a redner_b200 extension; by default the current PyTorch stream is used
@@ -530,28 +562,74 @@ def render(scene, options, rendered_image, d_rendered_image, d_scene, screen_gra
     same from run to run, at some cost in time and 88 bytes of device scratch per gradient float.  There is no other switch; every
     caller of this function (api.RenderFunction, api.SceneRenderer, api.render_batch, dist and the drop-in) follows PyTorch's."""
     lib = scene._lib
-    o = L.rb_options()
-    o.seed = options.seed
-    o.num_samples = options.num_samples
-    o.max_bounces = options.max_bounces
-    chs = (C.c_int * max(1, len(options.channels)))(*options.channels)
-    o.num_channels = len(options.channels)
-    o.channels = chs
-    o.sampler_type = options.sampler_type
-    o.sample_pixel_center = int(options.sample_pixel_center)
-    try:
-        import torch
-        o.deterministic = int(torch.are_deterministic_algorithms_enabled())
-    except ImportError:
-        o.deterministic = 0
-    if stream is None:
-        try:
-            import torch
-            # (the stream of the SCENE's device: a stream handle of another device would be invalid there)
-            stream = torch.cuda.current_stream(scene.gpu_index if scene.gpu_index >= 0 else None).cuda_stream if torch.cuda.is_available() else 0
-        except Exception:
-            stream = 0
+    o, _chs = _options(options)
     rc = lib.rb_render(scene._handle, C.byref(o), _addr(rendered_image) or None, _addr(d_rendered_image) or None,
-                       C.byref(d_scene._c) if d_scene is not None else None, _addr(screen_gradient_image) or None, C.c_void_p(stream or 0))
+                       C.byref(d_scene._c) if d_scene is not None else None, _addr(screen_gradient_image) or None, _render_stream(scene, stream))
     if rc != 0:
         raise RuntimeError("redner.render: " + L.last_error(lib))
+
+
+# --- exact records (redner_b200 extension, no reference counterpart): deterministic gradients summed across calls, devices and processes.
+# render_exact hands out the exact accumulators of a deterministic backward pass as an int64 tensor [count, RB_EXACT_RECORD_WORDS];
+# records of several calls -- the stripes of one image on several ranks -- are summed as integers (torch.distributed.all_reduce SUM,
+# or plain tensor addition), and round_exact turns the sum into gradients once: those of ONE deterministic render over all the
+# samples, bit for bit (include/redner_b200.h, rb_render_exact).
+
+def _scene_device(scene):
+    import torch
+    return torch.device("cuda", scene.gpu_index if scene.gpu_index >= 0 else torch.cuda.current_device()) if scene.use_gpu else torch.device("cpu")
+
+
+def exact_record_count(scene, options, d_scene, screen_gradient_image=None):
+    """(number of records, 64-bit fingerprint of their layout) of a backward pass of `options` into `d_scene` (rb_exact_record_count).
+    The fingerprint depends on the structure of the descriptor only; ranks compare it before they sum their records."""
+    lib = scene._lib
+    o, _chs = _options(options, True)
+    n, fp = C.c_size_t(0), C.c_uint64(0)
+    if lib.rb_exact_record_count(scene._handle, C.byref(o), C.byref(d_scene._c) if d_scene is not None else None, _addr(screen_gradient_image) or None,
+                                 C.byref(n), C.byref(fp)) != 0:
+        raise RuntimeError("redner.exact_record_count: " + L.last_error(lib))
+    return n.value, fp.value
+
+
+def _check_records(records, count, device, who):
+    import torch
+    if records is None:
+        raise RuntimeError("redner.%s: records is None" % who)
+    if records.dtype != torch.int64 or not records.is_contiguous() or records.device != device:
+        raise RuntimeError("redner.%s: records must be a contiguous int64 tensor on %s" % (who, device))
+    if records.numel() != count * L.RB_EXACT_RECORD_WORDS:
+        raise RuntimeError("redner.%s: records holds %d words, the descriptor needs %d records of %d" % (who, records.numel(), count, L.RB_EXACT_RECORD_WORDS))
+
+
+def render_exact(scene, options, d_rendered_image, d_scene, screen_gradient_image=None, records=None, stream=None):
+    """The deterministic backward pass of `render`, ending in records instead of gradients (rb_render_exact): returns `records` -- an
+    int64 tensor [count, RB_EXACT_RECORD_WORDS] on the scene's device, zeros if None -- with this pass's accumulators added.  No buffer of
+    `d_scene` is written; its pointers only give the layout."""
+    import torch
+    lib = scene._lib
+    count, _ = exact_record_count(scene, options, d_scene, screen_gradient_image)
+    dev = _scene_device(scene)
+    if records is None:
+        records = torch.zeros((count, L.RB_EXACT_RECORD_WORDS), dtype=torch.int64, device=dev)
+    _check_records(records, count, dev, "render_exact")
+    o, _chs = _options(options, True)
+    rc = lib.rb_render_exact(scene._handle, C.byref(o), _addr(d_rendered_image) or None, C.byref(d_scene._c), _addr(screen_gradient_image) or None,
+                             C.c_void_p(records.data_ptr()), count, _render_stream(scene, stream))
+    if rc != 0:
+        raise RuntimeError("redner.render_exact: " + L.last_error(lib))
+    return records
+
+
+def round_exact(scene, options, d_scene, screen_gradient_image, records, stream=None):
+    """The end of a deterministic `render` on `records` (a sum of render_exact results of this layout) (rb_exact_round): every record
+    that received something is rounded once and added into d_scene's buffers / the screen-gradient image, and the camera gradients are
+    finished with the scene's camera."""
+    lib = scene._lib
+    count, _ = exact_record_count(scene, options, d_scene, screen_gradient_image)
+    _check_records(records, count, _scene_device(scene), "round_exact")
+    o, _chs = _options(options, True)
+    rc = lib.rb_exact_round(scene._handle, C.byref(o), C.byref(d_scene._c), _addr(screen_gradient_image) or None, C.c_void_p(records.data_ptr()), count,
+                            _render_stream(scene, stream))
+    if rc != 0:
+        raise RuntimeError("redner.round_exact: " + L.last_error(lib))

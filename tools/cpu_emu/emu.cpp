@@ -361,8 +361,9 @@ extern "C" int rb_scene_last_stats(const rb_scene*, int* n, float* ms) {
     return 0;
 }
 
-extern "C" int rb_render(const rb_scene* scene, const rb_options* opt, float* image, const float* d_image, const rb_dscene_desc* d_scene,
-                         float* screen_grad, void*) {
+// rb_render (records == nullptr) and rb_render_exact (the accumulators are added into `records` instead of rounded), as in the library.
+static int emu_render(const rb_scene* scene, const rb_options* opt, float* image, const float* d_image, const rb_dscene_desc* d_scene, float* screen_grad,
+                      long long* records, size_t count) {
     if (!scene || !opt) {
         g_err = "rb_render: null scene / options";
         return 1;
@@ -417,7 +418,7 @@ extern "C" int rb_render(const rb_scene* scene, const rb_options* opt, float* im
         acc.base = cam_f.data();
         acc.stride = 1;
         // deterministic mode: every scatter and camera contribution into the exact accumulators of the library's layout
-        const bool det = opt->deterministic != 0;
+        const bool det = opt->deterministic != 0 || records != nullptr;
         ExactLayout xl;
         std::vector<long long> xacc;
         struct ExactReset {
@@ -431,6 +432,15 @@ extern "C" int rb_render(const rb_scene* scene, const rb_options* opt, float* im
         };
         if (det) {
             exact_layout(*d_scene, scene->shapes.data(), scene->materials.data(), sc, ka, xl);
+            if (records && xl.overlaps) {
+                g_err = "rb_render_exact: gradient buffers of d_scene overlap; records need disjoint buffers";
+                return 1;
+            }
+            if (records && (size_t)xl.num_records != count) {
+                g_err = "rb_render_exact: count is " + std::to_string(count) + " but the descriptor has " + std::to_string(xl.num_records) +
+                        " records (rb_exact_record_count)";
+                return 1;
+            }
             xacc.assign((size_t)(xl.num_acc + 1) * RB_EXACT_WORDS, 0);
             ka.ds.shapes = xl.shapes.data();
             ka.ds.materials = xl.materials.data();
@@ -476,9 +486,77 @@ extern "C" int rb_render(const rb_scene* scene, const rb_options* opt, float* im
                     exact_sample_done();
                 }
         }
+        if (records) {
+            for (long long i = 0; i < xl.num_acc; i++)
+                exact_export(&xacc[(size_t)i * RB_EXACT_WORDS],
+                             records + exact_record_of(i, xl.ranges.data(), xl.rec_first.data(), (int)xl.ranges.size(), RB_CAM_ACC) * RB_EXACT_RECORD_WORDS);
+            return 0;
+        }
         if (det)
             for (long long i = 0; i < xl.num_acc; i++) exact_finalise(xacc.data(), i, xl.ranges.data(), (int)xl.ranges.size(), cam_accum.data(), RB_CAM_ACC);
         finish_camera(sc.cam, cam_accum.data(), d_scene->camera);
     }
+    return 0;
+}
+extern "C" int rb_render(const rb_scene* scene, const rb_options* opt, float* image, const float* d_image, const rb_dscene_desc* d_scene,
+                         float* screen_grad, void*) {
+    return emu_render(scene, opt, image, d_image, d_scene, screen_grad, nullptr, 0);
+}
+extern "C" int rb_exact_record_count(const rb_scene* scene, const rb_options* opt, const rb_dscene_desc* d_scene, float* screen_grad, size_t* count,
+                                     uint64_t* fingerprint) {
+    if (!scene || !opt || !count) {
+        g_err = "rb_exact_record_count: null scene / options / count";
+        return 1;
+    }
+    KernelArgs ka;
+    ExactLayout xl;
+    std::string err;
+    if (const char* e = exact_record_layout("rb_exact_record_count", *opt, scene->cam, scene->max_generic, d_scene, screen_grad, scene->shapes.data(),
+                                            scene->materials.data(), scene->dev, ka, xl, err)) {
+        g_err = e;
+        return 1;
+    }
+    *count = (size_t)xl.num_records;
+    if (fingerprint) *fingerprint = xl.fingerprint;
+    return 0;
+}
+extern "C" int rb_render_exact(const rb_scene* scene, const rb_options* opt, const float* d_image, const rb_dscene_desc* d_scene, float* screen_grad,
+                               long long* records, size_t count, void*) {
+    if (!d_image || !d_scene || !records) {
+        g_err = "rb_render_exact: null d_rendered_image / d_scene / records";
+        return 1;
+    }
+    return emu_render(scene, opt, nullptr, d_image, d_scene, screen_grad, records, count);
+}
+extern "C" int rb_exact_round(const rb_scene* scene, const rb_options* opt, const rb_dscene_desc* d_scene, float* screen_grad, const long long* records,
+                              size_t count, void*) {
+    if (!scene || !opt || !records) {
+        g_err = "rb_exact_round: null scene / options / records";
+        return 1;
+    }
+    if (scene->incomplete) {
+        g_err = "rb_exact_round: the scene's last update failed; update it again or build a new scene";
+        return 1;
+    }
+    KernelArgs ka;
+    ExactLayout xl;
+    std::string err;
+    if (const char* e = exact_record_layout("rb_exact_round", *opt, scene->cam, scene->max_generic, d_scene, screen_grad, scene->shapes.data(),
+                                            scene->materials.data(), scene->dev, ka, xl, err)) {
+        g_err = e;
+        return 1;
+    }
+    if ((size_t)xl.num_records != count) {
+        g_err = "rb_exact_round: count is " + std::to_string(count) + " but the descriptor has " + std::to_string(xl.num_records) +
+                " records (rb_exact_record_count)";
+        return 1;
+    }
+    std::vector<long long> acc((size_t)(xl.num_acc + 1) * RB_EXACT_WORDS, 0);
+    std::vector<double> cam_accum(RB_CAM_ACC, 0.0);
+    for (long long i = 0; i < xl.num_acc; i++)
+        exact_import(records + exact_record_of(i, xl.ranges.data(), xl.rec_first.data(), (int)xl.ranges.size(), RB_CAM_ACC) * RB_EXACT_RECORD_WORDS,
+                     &acc[(size_t)i * RB_EXACT_WORDS]);
+    for (long long i = 0; i < xl.num_acc; i++) exact_finalise(acc.data(), i, xl.ranges.data(), (int)xl.ranges.size(), cam_accum.data(), RB_CAM_ACC);
+    finish_camera(scene->dev.cam, cam_accum.data(), d_scene->camera);
     return 0;
 }
