@@ -109,6 +109,17 @@ typedef struct rb_envmap {
     int directly_visible;
 } rb_envmap;
 
+/* Pixel reconstruction filter (no reference counterpart; the reference integrates radiance over the 1 x 1 pixel box).  Widths are in
+ * pixels: the box's side length; the tent's base width (radius width / 2); the Gaussian's truncation interval [-width / 2, width / 2],
+ * with sigma = width / 6.  The filter is separable and importance-sampled: a camera sample is placed at the pixel centre plus an offset
+ * drawn from the filter, and keeps weight 1 / num_samples, so a pixel is the filter-weighted integral of the radiance around its
+ * centre.  Samples may land outside their pixel and outside the image. */
+enum rb_filter_type { RB_FILTER_BOX = 0, RB_FILTER_TENT = 1, RB_FILTER_GAUSSIAN = 2 };
+typedef struct rb_pixel_filter {
+    int type;    /* rb_filter_type */
+    float width; /* in (0, 4] pixels; { 0, 0 } == { RB_FILTER_BOX, 1 } */
+} rb_pixel_filter;
+
 /* Scene -- constructor arguments of src/scene.cpp:63-75 / src/redner.cpp:62-73 */
 typedef struct rb_scene_desc {
     rb_camera camera;
@@ -123,6 +134,13 @@ typedef struct rb_scene_desc {
     int gpu_index;               /* -1 == current device (src/pathtracer.cpp:186-191) */
     int use_primary_edge_sampling;
     int use_secondary_edge_sampling;
+    /* A zero-initialised field is the 1-pixel box: the reference's image formation, bit for bit.  The filter belongs to the scene because
+     * the primary-edge distribution depends on its radius: it covers the image grown by max(0, width / 2 - 0.5) pixels on each side.
+     * rb_scene_create and rb_scene_update refuse, with a message naming the pixel filter, an unknown type, a width outside (0, 4], and any
+     * filter but the 1-pixel box with a fisheye or panorama camera or a lens-distortion model; rb_scene_set_camera refuses those
+     * cameras on a scene with such a filter.  rb_render refuses such a filter together with sample_pixel_center or a
+     * screen_gradient_image. */
+    rb_pixel_filter pixel_filter;
 } rb_scene_desc;
 
 /* RenderOptions -- src/pathtracer.h:16-23 */
@@ -197,8 +215,8 @@ int rb_scene_create_on_stream(const rb_scene_desc* desc, rb_scene** out, void* s
  * pdf_norm).
  * The build reads vertex positions in place, so an in-place write to them is invisible to the library: pass geometry_changed != 0
  * after one.  Then -- or when any `vertices` pointer changed -- the BVH, the light areas and area CDFs, the environment map's
- * bounding sphere, the edge list and the camera-dependent tables are rebuilt.  Otherwise, when the camera differs by value, only the
- * camera-dependent tables are, as rb_scene_set_camera does (but on the host for the small scenes whose build made them there, so
+ * bounding sphere, the edge list and the camera-dependent tables are rebuilt.  Otherwise, when the camera or the pixel filter differs by
+ * value, only the camera-dependent tables are, as rb_scene_set_camera does (but on the host for the small scenes whose build made them there, so
  * that they stay the build's tables byte for byte).  The shape / material descriptors, the lights and the light PMF / CDF are
  * refreshed on every call.
  * After a successful update every table of the scene is the one rb_scene_create would build from the same descriptor, byte for
@@ -224,7 +242,7 @@ int rb_render(const rb_scene* scene, const rb_options* options, float* rendered_
 
 /* Re-target a scene at another camera.  Only what depends on the camera is rebuilt, on the device: the primary-edge distribution
  * (src/edge.cpp:298-331) and the two secondary-edge trees (src/edge_tree.cpp:724-882); geometry, BVH, light tables and the edge
- * list are kept.  (The reference rebuilds the whole Scene per view, pyredner/render_pytorch.py:608-617.) */
+ * list are kept, and so is the scene's pixel filter.  (The reference rebuilds the whole Scene per view, pyredner/render_pytorch.py:608-617.) */
 int rb_scene_set_camera(rb_scene* scene, const rb_camera* camera);
 
 /* A batch of views of one scene -- the native form of the per-view Python loops of pyredner/render_utils.py:407-430 and of

@@ -72,6 +72,14 @@ class rb_envmap(C.Structure):
     ]
 
 
+# enum rb_filter_type
+RB_FILTER_BOX, RB_FILTER_TENT, RB_FILTER_GAUSSIAN = 0, 1, 2
+
+
+class rb_pixel_filter(C.Structure):
+    _fields_ = [("type", C.c_int), ("width", C.c_float)]
+
+
 class rb_scene_desc(C.Structure):
     _fields_ = [
         ("camera", rb_camera),
@@ -81,6 +89,7 @@ class rb_scene_desc(C.Structure):
         ("envmap", C.POINTER(rb_envmap)),
         ("use_gpu", C.c_int), ("gpu_index", C.c_int),
         ("use_primary_edge_sampling", C.c_int), ("use_secondary_edge_sampling", C.c_int),
+        ("pixel_filter", rb_pixel_filter),
     ]
 
 

@@ -181,6 +181,22 @@ class EnvironmentMap:
         self.sample_cdf_ys = ((cdf_ys_ - cdf_ys_[0]) / torch.clamp(cdf_ys_[-1], min=1e-8)).contiguous()
 
 
+class PixelFilter:
+    """Pixel reconstruction filter of a scene (redner_b200 extension; the reference integrates over the 1 x 1 pixel box).  `width` in
+    pixels: the box's side, the tent's base width, the Gaussian's truncation interval (sigma = width / 6); at most 4.  Passed as
+    `pixel_filter=` to serialize_scene and everything that forwards its options; None keeps the 1-pixel box."""
+    KINDS = ("box", "tent", "gaussian")  # rb_filter_type
+
+    def __init__(self, kind: str = "box", width: float = 1.0):
+        if kind not in self.KINDS:
+            raise ValueError("PixelFilter: kind must be one of %s, not %r" % (", ".join(self.KINDS), kind))
+        self.kind, self.width = kind, float(width)
+
+    def native(self):
+        """(rb_filter_type, width) as redner.Scene takes it."""
+        return self.KINDS.index(self.kind), self.width
+
+
 class Scene:
     def __init__(self, camera: Camera, shapes: List[Shape], materials: List[Material], area_lights: List[AreaLight], envmap=None):
         self.camera, self.shapes, self.materials, self.area_lights, self.envmap = camera, shapes, materials, area_lights, envmap
@@ -217,7 +233,7 @@ class RenderFunction(torch.autograd.Function):
     @staticmethod
     def serialize_scene(scene: Scene, num_samples: Union[int, Tuple[int, int]], max_bounces: int, channels=None, sampler_type=None,
                         use_primary_edge_sampling: bool = True, use_secondary_edge_sampling: bool = True, sample_pixel_center: bool = False,
-                        device: Optional[torch.device] = None, backend=None):
+                        device: Optional[torch.device] = None, backend=None, pixel_filter: Optional[PixelFilter] = None):
         backend = backend or default_backend()
         if channels is None:
             channels = [backend.channels.radiance]
@@ -275,7 +291,7 @@ class RenderFunction(torch.autograd.Function):
             args.append(None)
         args += [num_samples, max_bounces, channels, sampler_type]
         args += [use_primary_edge_sampling and vis, use_secondary_edge_sampling and vis]
-        args += [sample_pixel_center, device, backend]
+        args += [sample_pixel_center, pixel_filter.native() if pixel_filter is not None else None, device, backend]
         return args
 
     @staticmethod
@@ -310,7 +326,7 @@ class RenderFunction(torch.autograd.Function):
             env_mips = [nxt() for _ in range(n_env)]
             env_args = (env_mips, nxt(), nxt(), nxt(), nxt(), nxt(), nxt(), nxt())  # uv_scale, e2w, w2e, cdf_ys, cdf_xs, pdf_norm, visible
         num_samples, max_bounces, channels, sampler_type = nxt(), nxt(), nxt(), nxt()
-        use_prim, use_sec, pixel_center, device, backend = nxt(), nxt(), nxt(), nxt(), nxt()
+        use_prim, use_sec, pixel_center, pixel_filter, device, backend = nxt(), nxt(), nxt(), nxt(), nxt(), nxt()
         rb = backend
         fp, ip = (lambda t: _ptr(rb, t, "float")), (lambda t: _ptr(rb, t, "int"))
         camera = rb.Camera(resolution[1], resolution[0], fp(cam_pos if c2w is None else None), fp(cam_look if c2w is None else None),
@@ -343,11 +359,13 @@ class RenderFunction(torch.autograd.Function):
             mips, uv_scale, e2w, w2e, cdf_ys, cdf_xs, pdf_norm, visible = env_args
             env_tex = rb.Texture3([fp(m) for m in mips], [int(m.shape[1]) for m in mips], [int(m.shape[0]) for m in mips], 3, fp(uv_scale))
             envmap = rb.EnvironmentMap(env_tex, fp(e2w), fp(w2e), fp(cdf_ys), fp(cdf_xs), pdf_norm, visible)
-        c.env_args, c.envmap = env_args, envmap
+        c.env_args, c.envmap, c.pixel_filter = env_args, envmap, pixel_filter
         if scene is None:
-            c.scene = rb.Scene(camera, shapes, materials, lights, envmap, use_gpu, gpu_index, use_prim, use_sec)
+            # (the keyword only when a filter is set: a backend without pixel filters renders the 1-pixel box)
+            c.scene = rb.Scene(camera, shapes, materials, lights, envmap, use_gpu, gpu_index, use_prim, use_sec,
+                               **({} if pixel_filter is None else {"pixel_filter": pixel_filter}))
         elif geometry_changed is not None:
-            scene.update(camera, shapes, materials, lights, envmap, geometry_changed=geometry_changed)
+            scene.update(camera, shapes, materials, lights, envmap, geometry_changed=geometry_changed, pixel_filter=pixel_filter)
             c.scene = scene
         else:
             scene.set_camera(camera)
@@ -460,7 +478,7 @@ class RenderFunction(torch.autograd.Function):
             out += [g.envmap[1], None, g.envmap[2].cpu(), None, None, None, None]  # uv_scale, env_to_world, world_to_env, cdfs, pdf_norm, visible
         else:
             out.append(None)  # envmap
-        out += [None] * 9  # num_samples .. backend
+        out += [None] * 10  # num_samples .. backend
         return tuple(out)
 
     @staticmethod
@@ -562,8 +580,8 @@ class SceneRenderer:
         if k is not None:
             for _ in range(6):  # matrices, sampling tables, pdf_norm, directly_visible
                 nxt()
-        rest = [nxt() for _ in range(9)]
-        flags = (bool(rest[4]), bool(rest[5]), str(rest[7]))  # edge-sampling flags, device
+        rest = [nxt() for _ in range(10)]
+        flags = (bool(rest[4]), bool(rest[5]), str(rest[8]))  # edge-sampling flags, device
         return tuple(shapes), tuple(mats), tuple(lights), env, flags
 
     def _target(self, args):
@@ -628,7 +646,7 @@ class _SceneRenderFunction(torch.autograd.Function):
     def backward(ctx, grad_img):
         c = ctx.c
         if c.scene._generation != ctx.generation:  # updated since this forward pass: back to the state it rendered
-            c.scene.update(c.camera, c.shapes, c.materials, c.lights, c.envmap, geometry_changed=True)
+            c.scene.update(c.camera, c.shapes, c.materials, c.lights, c.envmap, geometry_changed=True, pixel_filter=c.pixel_filter)
             c.scene._generation += 1
             ctx.generation = c.scene._generation
         return (None,) + RenderFunction.backward(ctx, grad_img)
@@ -670,9 +688,9 @@ RenderFunction.visualize_screen_gradient = staticmethod(visualize_screen_gradien
 
 
 def render_pathtracing(scene: Scene, num_samples=(4, 4), max_bounces: int = 1, seed: int = 0, sampler_type=None, device=None, backend=None,
-                       use_primary_edge_sampling=True, use_secondary_edge_sampling=True):
+                       use_primary_edge_sampling=True, use_secondary_edge_sampling=True, pixel_filter: Optional[PixelFilter] = None):
     """pyredner.render_pathtracing (pyredner/render_utils.py:505-573) for a single scene."""
     args = RenderFunction.serialize_scene(scene, num_samples, max_bounces, sampler_type=sampler_type, device=device, backend=backend,
                                           use_primary_edge_sampling=use_primary_edge_sampling,
-                                          use_secondary_edge_sampling=use_secondary_edge_sampling)
+                                          use_secondary_edge_sampling=use_secondary_edge_sampling, pixel_filter=pixel_filter)
     return RenderFunction.apply(seed, *args)

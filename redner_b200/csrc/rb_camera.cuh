@@ -589,4 +589,41 @@ RB_HD bool cam_in_screen(const DevCamera& cam, V2 pt) {
     if (RB_CAM_GENERAL(cam) && cam.type == RB_CAMERA_FISHEYE) return rb_sq(pt.x - Real(0.5)) + rb_sq(pt.y - Real(0.5)) < Real(0.25); // src/camera.h:1059-1066
     return pt.x >= 0 && pt.x < 1 && pt.y >= 0 && pt.y < 1;
 }
+
+// ---- pixel reconstruction filter (rb_pixel_filter; DESIGN.md "pixel filters").  Separable: f(dx, dy) = f1(dx) f1(dy), offsets in pixels
+// from the pixel centre.  Cameras with a filter other than the 1-pixel box (RB_PIXEL_BOX) are linear: rb_scene_create refuses the rest.
+RB_HD double filter_radius(const DevCamera& cam) { return 0.5 * (double)cam.filter_width; }
+// Pixels by which the support of the viewport's pixels reaches past the viewport: the primary-edge distribution covers the image
+// grown by this much on each side.
+RB_HD double filter_grow(const DevCamera& cam) { return filter_radius(cam) > 0.5 ? filter_radius(cam) - 0.5 : 0.0; }
+// The Gaussian's sigma = width / 6, truncated at +-3 sigma: erf(r / (sigma sqrt 2)) = erf(3 / sqrt 2).
+#define RB_FILTER_GAUSS_ERF_R 0.99730020393673979
+// f1, normalised over its support (the 1-pixel box: 1).
+RB_HD double filter_density(const DevCamera& cam, double t) {
+    const double r = filter_radius(cam);
+    t = fabs(t);
+    if (!(t < r)) return 0.0;
+    if (cam.filter_type == RB_FILTER_TENT) return (r - t) / (r * r);
+    if (cam.filter_type == RB_FILTER_GAUSSIAN) {
+        const double sigma = (double)cam.filter_width / 6.0;
+        return exp(-t * t / (2.0 * sigma * sigma)) / (sigma * 2.50662827463100050 * RB_FILTER_GAUSS_ERF_R);
+    }
+    return 1.0 / (double)cam.filter_width;
+}
+// Inverse CDF of f1: u in [0, 1) -> offset from the pixel centre.
+RB_D double filter_offset(const DevCamera& cam, double u) {
+    const double r = filter_radius(cam);
+    if (cam.filter_type == RB_FILTER_TENT) return u < 0.5 ? r * (sqrt(2.0 * u) - 1.0) : r * (1.0 - sqrt(2.0 * (1.0 - u)));
+    if (cam.filter_type == RB_FILTER_GAUSSIAN) {
+        const double sigma = (double)cam.filter_width / 6.0;
+        return sigma * 1.41421356237309515 * erfinv((2.0 * u - 1.0) * RB_FILTER_GAUSS_ERF_R);
+    }
+    return (u - 0.5) * (double)cam.filter_width;
+}
+// A primary-edge point can reach a viewport pixel through the filter: the viewport grown by filter_grow (inside the grown image
+// the distribution covers).
+RB_HD bool cam_in_filter_reach(const DevCamera& cam, D2 pt) {
+    const double g = filter_grow(cam), x = pt.x * cam.width, y = pt.y * cam.height;
+    return x >= cam.vp_beg[0] - g && x < cam.vp_end[0] + g && y >= cam.vp_beg[1] - g && y < cam.vp_end[1] + g;
+}
 RB_HD bool ray_is_null(const Ray& r) { return r.dir.x == 0 && r.dir.y == 0 && r.dir.z == 0; }

@@ -123,12 +123,18 @@ static int render_pass(const rb_scene* scene_, const rb_options* opt, float* ima
         rb_set_error(err);
         return 1;
     }
+    if (const char* err = check_pixel_filter_options(scene->dev.cam, *opt, screen_grad)) {
+        rb_set_error(err);
+        return 1;
+    }
     const RenderParams& rp = ka.rp;
     if (rp.vp_w <= 0 || rp.vp_h <= 0 || rp.spp == 0) return 0;
     // The feature-free instantiation of the kernels (rb_kernels_lean.cu) serves the common configuration; `kern` holds the kernels of
     // the chosen instantiation, and every launch of one of them below goes through it.
     const bool lean_allowed = getenv("RB_NO_LEAN") == nullptr; // (test hook: force the general kernels)
-    const bool lean = lean_allowed && rp.only_radiance && !scene->dev.has_envmap && scene->dev.cam.type == RB_CAMERA_PERSPECTIVE && !scene->dev.cam.has_distortion;
+    const DevCamera& cam = scene->dev.cam;
+    const bool lean = lean_allowed && rp.only_radiance && !scene->dev.has_envmap && cam.type == RB_CAMERA_PERSPECTIVE && !cam.has_distortion &&
+                      cam.filter_type == RB_FILTER_BOX && cam.filter_width == 1.0f;
     const RenderKernels kern = lean ? rb_lean::render_kernels() : render_kernels();
     // Deterministic mode: the backward kernels of rb_kernels_det.cu (the forward kernels are deterministic as they are).  Records
     // come from the exact accumulators, so rb_render_exact runs them whatever the options say.

@@ -32,18 +32,20 @@ typedef float Real;
 #define RB_DFN inline __device__ __noinline__
 
 // Feature tests.  rb_kernels_lean.cu compiles the same kernels a second time with RB_LEAN defined: no environment map, pinhole
-// camera without lens model, channels == [radiance] -- the configuration of nearly every optimisation loop.  There the
-// tests are compile-time constants and the rarely used code disappears from the instruction stream (DESIGN.md section 2).
+// camera without lens model, channels == [radiance], 1-pixel box filter -- the configuration of nearly every optimisation loop.
+// There the tests are compile-time constants and the rarely used code disappears from the instruction stream (DESIGN.md section 2).
 #ifdef RB_LEAN
 #define RB_ENVMAP(sc) false
 #define RB_CAM_GENERAL(cam) false
 #define RB_CAM_DISTORT(cam) false
 #define RB_ONLY_RADIANCE(rp) true
+#define RB_PIXEL_BOX(cam) true
 #else
 #define RB_ENVMAP(sc) ((sc).has_envmap != 0)
 #define RB_CAM_GENERAL(cam) ((cam).type != RB_CAMERA_PERSPECTIVE || (cam).has_distortion != 0)
 #define RB_CAM_DISTORT(cam) ((cam).has_distortion != 0)
 #define RB_ONLY_RADIANCE(rp) ((rp).only_radiance != 0)
+#define RB_PIXEL_BOX(cam) ((cam).filter_type == RB_FILTER_BOX && (cam).filter_width == 1.0f)
 #endif
 
 #ifndef M_PI

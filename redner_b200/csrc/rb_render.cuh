@@ -123,6 +123,13 @@ inline const char* setup_kernel_args(const rb_options& opt, const rb_camera& cam
     ka.screen_grad = screen_grad;
     return nullptr;
 }
+// rb_render's refusals under a pixel filter other than the 1-pixel box; returns the error message, or null.
+inline const char* check_pixel_filter_options(const DevCamera& cam, const rb_options& opt, const float* screen_grad) {
+    if (cam.filter_type == RB_FILTER_BOX && cam.filter_width == 1.0f) return nullptr;
+    if (opt.sample_pixel_center) return "rb_render: sample_pixel_center needs the 1-pixel box pixel filter (the scene's filter places samples around the centre)";
+    if (screen_grad != nullptr) return "rb_render: a screen_gradient_image needs the 1-pixel box pixel filter";
+    return nullptr;
+}
 // The boundary (secondary-edge) stage of the backward pass runs: it needs edges, a light and a radiance channel.
 RB_HD bool boundary_stage_runs(const DevScene& sc, const RenderParams& rp) {
     return sc.use_secondary_edge && sc.num_edges > 0 && sc.num_lights > 0 && rp.rad_dim >= 0;
@@ -182,12 +189,18 @@ RB_HD unsigned long long edge_draws_per_sample(const DevScene& sc, const RenderP
     return (unsigned long long)(primary_edge_dim_base(sc, rp) + 2 + 7 * rp.max_bounces);
 }
 
-// Screen position of a pixel sample: consumes the first two sampler dimensions unless sample_pixel_center.
+// Screen position of a pixel sample: consumes the first two sampler dimensions unless sample_pixel_center.  Under a pixel filter
+// other than the 1-pixel box each of the two numbers becomes an offset from the pixel centre through the filter's inverse CDF
+// (rb_render refuses sample_pixel_center there); the 1-pixel box keeps its own expression, which rounds differently.
 RB_D void primary_sample_pos(const DevScene& sc, const RenderParams& rp, int px, int py, Sampler& smp, double& sx, double& sy) {
     double jx = 0.5, jy = 0.5;
     if (!rp.sample_pixel_center) {
         jx = smp.next();
         jy = smp.next();
+    }
+    if (!RB_PIXEL_BOX(sc.cam)) {
+        jx = 0.5 + filter_offset(sc.cam, jx);
+        jy = 0.5 + filter_offset(sc.cam, jy);
     }
     sx = (double(px + sc.cam.vp_beg[0]) + jx) / double(sc.cam.width);
     sy = (double(py + sc.cam.vp_beg[1]) + jy) / double(sc.cam.height);
@@ -730,7 +743,7 @@ RB_D bool primary_edge_pick(const DevScene& sc, const RenderParams& rp, long lon
     if (cam_is_linear(sc.cam)) {
         pk.ept.x = pk.q0.x + pk.e_t * (pk.q1.x - pk.q0.x);
         pk.ept.y = pk.q0.y + pk.e_t * (pk.q1.y - pk.q0.y);
-        if (!cam_in_screen(sc.cam, mk2((Real)pk.ept.x, (Real)pk.ept.y))) return false;
+        if (RB_PIXEL_BOX(sc.cam) ? !cam_in_screen(sc.cam, mk2((Real)pk.ept.x, (Real)pk.ept.y)) : !cam_in_filter_reach(sc.cam, pk.ept)) return false;
         // unit normal of the projected edge: get_normal(normalize(v0_ss - v1_ss)) = (d.y, -d.x); rays at +-1e-6 across it
         double ddx = pk.q0.x - pk.q1.x, ddy = pk.q0.y - pk.q1.y;
         double dl = sqrt(ddx * ddx + ddy * ddy);
@@ -757,6 +770,25 @@ RB_D unsigned primary_edge_key(const DevScene& sc, const RenderParams& rp, long 
     unsigned tq = tbits > 0 ? (unsigned)rb_clampi((int)(pk.e_t * (double)(1u << tbits)), 0, (1 << tbits) - 1) : 0u;
     return ((unsigned)pk.edge_id << tbits) | tq;
 }
+// out[0, nd) = sum of f(p - c) d_image[c] over the viewport pixels c whose filter support holds the screen point p (at most 4 x 4 of
+// them for widths up to 4 pixels), in a fixed order.
+RB_D void filter_splat(const DevCamera& cam, const RenderParams& rp, const float* d_image, D2 p, float* out) {
+    const int nd = rp.nd < RB_MAX_ND ? rp.nd : RB_MAX_ND;
+    for (int k = 0; k < nd; k++) out[k] = 0.f;
+    const double r = filter_radius(cam);
+    // offsets from the centre of viewport pixel (0, 0); pixel c is reached when |offset - c| < r
+    const double x = p.x * cam.width - cam.vp_beg[0] - 0.5, y = p.y * cam.height - cam.vp_beg[1] - 0.5;
+    const int cx0 = rb_clampi((int)floor(x - r) + 1, 0, rp.vp_w), cx1 = rb_clampi((int)ceil(x + r) - 1, -1, rp.vp_w - 1);
+    const int cy0 = rb_clampi((int)floor(y - r) + 1, 0, rp.vp_h), cy1 = rb_clampi((int)ceil(y + r) - 1, -1, rp.vp_h - 1);
+    for (int cy = cy0; cy <= cy1; cy++) {
+        const double wy = filter_density(cam, y - cy);
+        for (int cx = cx0; cx <= cx1; cx++) {
+            const float w = (float)(wy * filter_density(cam, x - cx));
+            const float* px = d_image + (size_t)rp.nd * ((size_t)cy * rp.vp_w + cx);
+            for (int k = 0; k < nd; k++) out[k] += w * px[k];
+        }
+    }
+}
 RB_D void primary_edge_sample(const DevScene& sc, const KernelArgs& ka, long long i, int s, int dim_base, CamAcc& cam_acc) {
     const RenderParams& rp = ka.rp;
     const DevDScene& ds = ka.ds;
@@ -772,6 +804,13 @@ RB_D void primary_edge_sample(const DevScene& sc, const KernelArgs& ka, long lon
     int xi = rb_clampi(int(ept.x * sc.cam.width - sc.cam.vp_beg[0]), 0, sc.cam.vp_end[0] - sc.cam.vp_beg[0]);
     int yi = rb_clampi(int(ept.y * sc.cam.height - sc.cam.vp_beg[1]), 0, sc.cam.vp_end[1] - sc.cam.vp_beg[1]);
     const float* dpx_all = ka.d_image + (size_t)rp.nd * ((size_t)yi * vp_w + xi);
+    // Under a pixel filter the edge point weighs into every viewport pixel whose support holds it.  The integrand is linear in the
+    // d_image multipliers, so the rays and the scatter below run once, on their filter-weighted sum.
+    float d_splat[RB_MAX_ND];
+    if (!RB_PIXEL_BOX(sc.cam)) {
+        filter_splat(sc.cam, rp, ka.d_image, ept, d_splat);
+        dpx_all = d_splat;
+    }
     const float* dpx = dpx_all + (rp.rad_dim >= 0 ? rp.rad_dim : 0);
     V3 d_color = rp.rad_dim >= 0 ? mk3(dpx[0], dpx[1], dpx[2]) : zero3();
     V3 wgt = d_color * (Real)(pk.jacobian / pmf);

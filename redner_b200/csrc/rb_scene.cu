@@ -487,6 +487,7 @@ static int camera_step(rb_scene* sc, const rb_camera& cam, bool like_build, cuda
 static int scene_apply(rb_scene* sc, const rb_scene_desc& desc, bool geometry, bool camera, cudaStream_t stream) {
     sc->incomplete = true;
     sc->stream = stream;
+    host_setup_pixel_filter(desc.pixel_filter, sc->dev.cam); // (before the camera tables, whose clipping depends on it)
     sc->shapes.assign(desc.shapes, desc.shapes + desc.num_shapes);
     sc->materials.assign(desc.materials, desc.materials + desc.num_materials);
     sc->lights = host_area_lights(desc);
@@ -594,7 +595,9 @@ extern "C" int rb_scene_update(rb_scene* sc, const rb_scene_desc* desc, int geom
     // the host, they are made on the host again)
     bool geometry = geometry_changed != 0 || sc->incomplete;
     for (int s = 0; s < desc->num_shapes; s++) geometry = geometry || desc->shapes[s].vertices != sc->shapes[s].vertices;
-    const bool camera = memcmp(&desc->camera, &sc->cam, sizeof(rb_camera)) != 0 || !sc->camera_tables_as_built;
+    const rb_pixel_filter filter = host_pixel_filter(desc->pixel_filter);
+    const bool camera = memcmp(&desc->camera, &sc->cam, sizeof(rb_camera)) != 0 || !sc->camera_tables_as_built ||
+                        filter.type != sc->dev.cam.filter_type || filter.width != sc->dev.cam.filter_width;
     int prev = 0;
     cudaGetDevice(&prev);
     if (cudaSetDevice(sc->device) != cudaSuccess) {
@@ -764,6 +767,11 @@ extern "C" int rb_scene_set_camera(rb_scene* sc, const rb_camera* cam) {
     }
     if (sc->incomplete) {
         rb_set_error("rb_scene_set_camera: the scene's last update failed; update it again or build a new scene");
+        return 1;
+    }
+    if (const char* err = host_check_filter_camera(rb_pixel_filter{sc->dev.cam.filter_type, sc->dev.cam.filter_width}, *cam)) {
+        rb_set_error(err);
+        retitle_error("rb_scene_set_camera");
         return 1;
     }
     int prev = 0;

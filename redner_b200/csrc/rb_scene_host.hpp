@@ -32,8 +32,32 @@ struct HostEdgeTables {
 };
 
 // ---- scene descriptor -> scene, shared by both rb_scene_create (rb_scene.cu and the emulator's)
-// Index checks of the descriptor; returns the error message, or null.
+// The pixel filter as the kernels see it: { 0, 0 } is the 1-pixel box.
+inline rb_pixel_filter host_pixel_filter(const rb_pixel_filter& f) {
+    if (f.type == 0 && f.width == 0.f) return rb_pixel_filter{RB_FILTER_BOX, 1.f};
+    return f;
+}
+inline bool host_pixel_box(const rb_pixel_filter& f) { return f.type == RB_FILTER_BOX && f.width == 1.f; }
+// A camera the primary-edge pass of a pixel filter other than the 1-pixel box handles: linear projection, no lens model.
+inline const char* host_check_filter_camera(const rb_pixel_filter& f, const rb_camera& cam) {
+    if (!host_pixel_box(host_pixel_filter(f)) && (cam.camera_type == RB_CAMERA_FISHEYE || cam.camera_type == RB_CAMERA_PANORAMA || cam.has_distortion))
+        return "rb_scene_create: pixel filters other than the 1-pixel box need a perspective or orthographic camera without lens distortion";
+    return nullptr;
+}
+inline const char* host_check_pixel_filter(const rb_scene_desc& desc) {
+    const rb_pixel_filter f = host_pixel_filter(desc.pixel_filter);
+    if (f.type != RB_FILTER_BOX && f.type != RB_FILTER_TENT && f.type != RB_FILTER_GAUSSIAN) return "rb_scene_create: unknown pixel filter type";
+    if (!(f.width > 0.f && f.width <= 4.f)) return "rb_scene_create: pixel filter width must lie in (0, 4] pixels";
+    return host_check_filter_camera(f, desc.camera);
+}
+inline void host_setup_pixel_filter(const rb_pixel_filter& f, DevCamera& dc) {
+    const rb_pixel_filter g = host_pixel_filter(f);
+    dc.filter_type = g.type;
+    dc.filter_width = g.width;
+}
+// Index and pixel-filter checks of the descriptor; returns the error message, or null.
 inline const char* host_check_scene_desc(const rb_scene_desc& desc) {
+    if (const char* err = host_check_pixel_filter(desc)) return err;
     for (int l = 0; l < desc.num_lights; l++)
         if (desc.lights[l].shape_id < 0 || desc.lights[l].shape_id >= desc.num_shapes) return "rb_scene_create: area light refers to an invalid shape";
     for (int s = 0; s < desc.num_shapes; s++) {

@@ -68,6 +68,9 @@ struct DevCamera {
     int vp_beg[2], vp_end[2];
     int has_distortion;   // Brown-Conrady lens model, src/camera_distortion.h
     double distortion[8]; // k1..k6 (radial, rational), p1, p2 (tangential)
+    // the scene's pixel filter (rb_scene_desc::pixel_filter, { 0, 0 } made { RB_FILTER_BOX, 1 }); rb_scene_set_camera keeps it
+    int filter_type;
+    float filter_width;
 };
 
 // ---- BVH (own LBVH; replaces Embree/OptiX Prime) ----

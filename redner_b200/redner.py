@@ -308,7 +308,8 @@ def compute_num_channels(chs, max_generic_texture_dimension):  # src/redner.cpp:
 
 class Scene:  # src/redner.cpp:62-73, src/scene.cpp:63-307
     def __init__(self, camera, shapes, materials, area_lights, envmap, use_gpu, gpu_index, use_primary_edge_sampling,
-                 use_secondary_edge_sampling):
+                 use_secondary_edge_sampling, pixel_filter=None):
+        """`pixel_filter` (redner_b200 extension): None for the 1-pixel box of the reference, or (rb_filter_type, width in pixels)."""
         lib = L.load()
         self._lib = lib
         self._handle = None
@@ -329,7 +330,7 @@ class Scene:  # src/redner.cpp:62-73, src/scene.cpp:63-307
         self.use_gpu = bool(use_gpu)
         self.gpu_index = int(gpu_index)
         self._flags = (int(bool(use_primary_edge_sampling)), int(bool(use_secondary_edge_sampling)))
-        d = self._desc(camera, shapes, materials, area_lights, envmap)
+        d = self._desc(camera, shapes, materials, area_lights, envmap, pixel_filter)
         h = C.c_void_p()
         stream = self._stream()
         if hasattr(lib, "rb_scene_create_on_stream"):
@@ -341,7 +342,7 @@ class Scene:  # src/redner.cpp:62-73, src/scene.cpp:63-307
         self._handle = h
         self.max_generic_texture_dimension = lib.rb_scene_max_generic_texture_dimension(h)
 
-    def _desc(self, camera, shapes, materials, area_lights, envmap):
+    def _desc(self, camera, shapes, materials, area_lights, envmap, pixel_filter):
         d = L.rb_scene_desc()
         d.camera = camera._c
         self._shapes = (L.rb_shape * max(1, len(shapes)))(*[s._c for s in shapes])
@@ -355,6 +356,8 @@ class Scene:  # src/redner.cpp:62-73, src/scene.cpp:63-307
         d.use_gpu = int(self.use_gpu)
         d.gpu_index = self.gpu_index
         d.use_primary_edge_sampling, d.use_secondary_edge_sampling = self._flags
+        if pixel_filter is not None:
+            d.pixel_filter = L.rb_pixel_filter(int(pixel_filter[0]), float(pixel_filter[1]))
         return d
 
     def _stream(self):
@@ -377,11 +380,11 @@ class Scene:  # src/redner.cpp:62-73, src/scene.cpp:63-307
         if self._lib.rb_scene_set_camera(self._handle, C.byref(camera._c)) != 0:
             raise RuntimeError("redner.Scene.set_camera: " + L.last_error(self._lib))
 
-    def update(self, camera, shapes, materials, area_lights, envmap, geometry_changed=True):
-        """Re-target this scene at shapes / materials / lights / environment map / camera of the SAME structure as its build, without
-        building a new scene (rb_scene_update): counts, ids and optional buffers as before, index buffers with the same contents.  Pass
-        geometry_changed=True when vertex positions may have been written in place; a new vertex buffer is noticed by itself."""
-        d = self._desc(camera, shapes, materials, area_lights, envmap)
+    def update(self, camera, shapes, materials, area_lights, envmap, geometry_changed=True, pixel_filter=None):
+        """Re-target this scene at shapes / materials / lights / environment map / camera / pixel filter of the SAME structure as its build,
+        without building a new scene (rb_scene_update): counts, ids and optional buffers as before, index buffers with the same contents.
+        Pass geometry_changed=True when vertex positions may have been written in place; a new vertex buffer is noticed by itself."""
+        d = self._desc(camera, shapes, materials, area_lights, envmap, pixel_filter)
         if self._lib.rb_scene_update(self._handle, C.byref(d), int(bool(geometry_changed)), C.c_void_p(self._stream() or 0)) != 0:
             raise RuntimeError("redner.Scene.update: " + L.last_error(self._lib))
 

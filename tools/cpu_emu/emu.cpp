@@ -94,6 +94,7 @@ static int emu_build(rb_scene* sc, const rb_scene_desc* desc) {
     d.sobol_dims = 1024;
     sc->cam = desc->camera;
     host_setup_camera(desc->camera, d.cam);
+    host_setup_pixel_filter(desc->pixel_filter, d.cam);
     sc->shapes.assign(desc->shapes, desc->shapes + desc->num_shapes);
     sc->materials.assign(desc->materials, desc->materials + desc->num_materials);
     sc->lights = host_area_lights(*desc);
@@ -318,6 +319,10 @@ extern "C" int rb_scene_edge_list(const rb_scene* sc, int* num_edges, int* edges
 // builders; geometry, BVH, lights and the edge list are kept (mirrors rb_scene_set_camera of the product, which rebuilds them on the GPU).
 extern "C" int rb_scene_set_camera(rb_scene* sc, const rb_camera* cam) {
     DevScene& d = sc->dev;
+    if (const char* err = host_check_filter_camera(rb_pixel_filter{d.cam.filter_type, d.cam.filter_width}, *cam)) {
+        g_err = std::string("rb_scene_set_camera:") + (err + 16);
+        return 1;
+    }
     sc->cam = *cam;
     host_setup_camera(*cam, d.cam);
     if (d.num_edges > 0) {
@@ -375,6 +380,10 @@ static int emu_render(const rb_scene* scene, const rb_options* opt, float* image
     KernelArgs ka;
     if (const char* err = setup_kernel_args(*opt, scene->cam, scene->max_generic, scene->part, scene->num_parts, scene->rps, image, d_image, d_scene,
                                             screen_grad, ka)) {
+        g_err = err;
+        return 1;
+    }
+    if (const char* err = check_pixel_filter_options(scene->dev.cam, *opt, screen_grad)) {
         g_err = err;
         return 1;
     }
