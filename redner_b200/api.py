@@ -11,6 +11,8 @@ Same names, argument meaning and error behaviour as the reference's Python layer
 unmodified reference module (oracle/_ref) through the very same host code to obtain the oracle's images and gradients.
 """
 import math
+from collections import namedtuple
+from types import SimpleNamespace
 from typing import List, Optional, Tuple, Union
 
 import torch
@@ -202,13 +204,75 @@ class Scene:
         self.camera, self.shapes, self.materials, self.area_lights, self.envmap = camera, shapes, materials, area_lights, envmap
 
 
-class _Ctx:
-    pass
+# The entries serialize_scene writes for one camera, shape, texture, material, light, environment map and the options, in their order
+# (RenderFunction.read_args).
+_CameraArgs = namedtuple("_CameraArgs", "position look_at up cam_to_world world_to_cam intrinsic_mat_inv intrinsic_mat distortion_params clip_near "
+                                        "resolution viewport camera_type")
+_ShapeArgs = namedtuple("_ShapeArgs", "vertices indices uvs normals uv_indices normal_indices colors material_id light_id")
+_TextureArgs = namedtuple("_TextureArgs", "mips uv_scale")
+_MaterialArgs = namedtuple("_MaterialArgs", "textures compute_specular_lighting two_sided use_vertex_color")
+_LightArgs = namedtuple("_LightArgs", "shape_id intensity two_sided directly_visible")
+_EnvmapArgs = namedtuple("_EnvmapArgs", "values env_to_world world_to_env sample_cdf_ys sample_cdf_xs pdf_norm directly_visible")
+_OptionArgs = namedtuple("_OptionArgs", "num_samples max_bounces channels sampler_type use_primary_edge_sampling use_secondary_edge_sampling "
+                                        "sample_pixel_center pixel_filter device backend")
 
 
 def _ptr(backend, t, kind="float"):
     ctor = backend.float_ptr if kind == "float" else backend.int_ptr
     return ctor(t.data_ptr() if t is not None else 0)
+
+
+def _native_texture(rb, cls, channels, tex, buffers=None):
+    """rb.Texture1 / Texture3 / TextureN of the texture entry `tex` of read_args (None: no texture, of `channels` channels), pointing at
+    the texture's own tensors, or at `buffers` = (mips, uv_scale) of the same shapes: its gradient."""
+    if tex is None:
+        return cls([], [], [], channels, rb.float_ptr(0))
+    mips, uv_scale = buffers or (tex.mips, tex.uv_scale)
+    first = tex.mips[0]
+    if first.dim() == 3:
+        return cls([_ptr(rb, m) for m in mips], [int(m.shape[1]) for m in tex.mips], [int(m.shape[0]) for m in tex.mips], int(first.shape[2]),
+                   _ptr(rb, uv_scale))
+    return cls([_ptr(rb, mips[0])], [0], [0], int(first.shape[0]), _ptr(rb, uv_scale))
+
+
+def _material_textures(rb):
+    """(class, channels of an absent texture) of a material's textures, in the order of read_args: diffuse, specular, roughness,
+    generic, normal map."""
+    return (rb.Texture3, 3), (rb.Texture3, 3), (rb.Texture1, 1), (rb.TextureN, 0), (rb.Texture3, 3)
+
+
+def _image_shape(c):
+    """(height, width, channels) of the image of the unpacked call `c`."""
+    vp = c.viewport
+    return vp[2] - vp[0], vp[3] - vp[1], c.backend.compute_num_channels(c.channels, c.scene.max_generic_texture_dimension)
+
+
+def _render(c):
+    """The image of the unpacked call `c`, rendered into a new zeroed tensor."""
+    rb = c.backend
+    img = torch.zeros(*_image_shape(c), device=c.device)
+    rb.render(c.scene, c.options, rb.float_ptr(img.data_ptr()), rb.float_ptr(0), None, rb.float_ptr(0), rb.float_ptr(0))
+    return img
+
+
+def _backward(c, grad_img, screen_grad=None):
+    """The backward pass of the unpacked call `c` for d(loss)/d(image) `grad_img`: the gradient of every argument of `c`, at its position
+    in RenderFunction.apply's arguments (RenderFunction.backward's return value).  `screen_grad`, an [height, width, 2] tensor, also
+    receives d(image)/d(screen position of each pixel)."""
+    rb = c.backend
+    grad_img = grad_img.contiguous()
+    assert torch.isfinite(grad_img).all()
+    g = RenderFunction.gradient_buffers(c)
+    rb.render(c.scene, RenderFunction.backward_options(c), rb.float_ptr(0), _ptr(rb, grad_img), g.d_scene, _ptr(rb, screen_grad), rb.float_ptr(0))
+    return RenderFunction.gradient_outputs(c, g)
+
+
+def _seeds(seed):
+    """The (forward, backward) seeds of RenderFunction.apply's `seed`."""
+    assert isinstance(seed, (tuple, int))
+    if isinstance(seed, tuple):
+        return seed
+    return seed, seed if _use_correlated_random_number else seed + 1000003
 
 
 def _serialize_texture(tex, args, device):
@@ -295,155 +359,155 @@ class RenderFunction(torch.autograd.Function):
         return args
 
     @staticmethod
+    def read_args(args):
+        """serialize_scene's argument list, read in one pass.  Besides serialize_scene, this is the only code that knows the list's layout.
+
+        Returns a namespace of `camera_args`, `shape_args`, `mat_args`, `light_args` (lists), `env_args` (None without an environment map)
+        and `option_args`: the entries serialize_scene wrote for each, as the named tuples above.  A material's `textures` are five
+        _TextureArgs or None (diffuse, specular, roughness, generic, normal map); the environment map's `values` is one.  `pos` holds the
+        same structure with the position in `args` of each entry in place of the entry.  `args` is the list itself."""
+        k = 3  # (after the numbers of shapes, materials and lights)
+
+        def entries(n):
+            nonlocal k
+            k += n
+            return args[k - n:k], range(k - n, k)
+
+        def take(cls):
+            values, positions = entries(len(cls._fields))
+            return cls._make(values), cls._make(positions)
+
+        def texture():
+            n, _ = entries(1)  # number of mip levels: 0 for a material without this texture, None for a scene without an environment map
+            if not n[0]:
+                return None, None
+            (mips, mip_pos), (uv, uv_pos) = entries(n[0]), entries(1)
+            return _TextureArgs(list(mips), uv[0]), _TextureArgs(list(mip_pos), uv_pos[0])
+
+        def material():
+            textures = [texture() for _ in range(5)]
+            values, positions = entries(3)
+            return _MaterialArgs([t for t, _ in textures], *values), _MaterialArgs([p for _, p in textures], *positions)
+
+        def each(n, read):
+            pairs = [read() for _ in range(n)]
+            return [v for v, _ in pairs], [p for _, p in pairs]
+
+        a = SimpleNamespace(args=args, pos=SimpleNamespace())
+        a.camera_args, a.pos.camera_args = take(_CameraArgs)
+        a.shape_args, a.pos.shape_args = each(args[0], lambda: take(_ShapeArgs))
+        a.mat_args, a.pos.mat_args = each(args[1], material)
+        a.light_args, a.pos.light_args = each(args[2], lambda: take(_LightArgs))
+        a.env_args = a.pos.env_args = None
+        values, positions = texture()
+        if values is not None:
+            rest, rest_pos = entries(len(_EnvmapArgs._fields) - 1)
+            a.env_args, a.pos.env_args = _EnvmapArgs(values, *rest), _EnvmapArgs(positions, *rest_pos)
+        a.option_args, a.pos.option_args = take(_OptionArgs)
+        assert k == len(args), "serialize_scene's list has %d entries, its layout %d" % (len(args), k)
+        return a
+
+    @staticmethod
     def _unpack(seed, args, scene=None, geometry_changed=None):
         """`scene`: an existing native scene of the SAME geometry / materials / lights to re-target at this argument list's camera
         (rb_scene_set_camera) instead of building a new one -- the batch path.  With `geometry_changed` (True / False) the scene only
-        needs the same structure and is re-targeted at everything in the argument list (Scene.update) -- the SceneRenderer path."""
-        it = iter(args)
-        nxt = lambda: next(it)  # noqa: E731
-        c = _Ctx()
-        num_shapes, num_materials, num_lights = nxt(), nxt(), nxt()
-        cam_pos, cam_look, cam_up, c2w, w2c, intr_inv, intr, dist = nxt(), nxt(), nxt(), nxt(), nxt(), nxt(), nxt(), nxt()
-        clip_near, resolution, viewport, camera_type = nxt(), nxt(), nxt(), nxt()
-        shape_args, mat_args, light_args = [], [], []
-        for _ in range(num_shapes):
-            shape_args.append([nxt() for _ in range(9)])
-        for _ in range(num_materials):
-            texs = []
-            for _ in range(5):
-                n = nxt()
-                if n == 0:
-                    texs.append(None)
-                else:
-                    mips = [nxt() for _ in range(n)]
-                    texs.append((mips, nxt()))
-            mat_args.append((texs, nxt(), nxt(), nxt()))
-        for _ in range(num_lights):
-            light_args.append([nxt() for _ in range(4)])
-        env_args = None
-        n_env = nxt()
-        if n_env is not None:
-            env_mips = [nxt() for _ in range(n_env)]
-            env_args = (env_mips, nxt(), nxt(), nxt(), nxt(), nxt(), nxt(), nxt())  # uv_scale, e2w, w2e, cdf_ys, cdf_xs, pdf_norm, visible
-        num_samples, max_bounces, channels, sampler_type = nxt(), nxt(), nxt(), nxt()
-        use_prim, use_sec, pixel_center, pixel_filter, device, backend = nxt(), nxt(), nxt(), nxt(), nxt(), nxt()
-        rb = backend
+        needs the same structure and is re-targeted at everything in the argument list (Scene.update) -- the SceneRenderer path.
+        Returns read_args(args) with the native objects built from it added."""
+        c = RenderFunction.read_args(args)
+        cam, opt = c.camera_args, c.option_args
+        rb, device, vp = opt.backend, opt.device, cam.viewport
         fp, ip = (lambda t: _ptr(rb, t, "float")), (lambda t: _ptr(rb, t, "int"))
-        camera = rb.Camera(resolution[1], resolution[0], fp(cam_pos if c2w is None else None), fp(cam_look if c2w is None else None),
-                           fp(cam_up if c2w is None else None), fp(c2w), fp(w2c), fp(intr_inv), fp(intr), fp(dist), clip_near,
-                           rb.CameraType(int(camera_type)),
-                           rb.Vector2i(viewport[1], viewport[0]), rb.Vector2i(viewport[3], viewport[2]))
+        look_at = cam.cam_to_world is None
+        camera = rb.Camera(cam.resolution[1], cam.resolution[0], fp(cam.position if look_at else None), fp(cam.look_at if look_at else None),
+                           fp(cam.up if look_at else None), fp(cam.cam_to_world), fp(cam.world_to_cam), fp(cam.intrinsic_mat_inv),
+                           fp(cam.intrinsic_mat), fp(cam.distortion_params), cam.clip_near, rb.CameraType(int(cam.camera_type)),
+                           rb.Vector2i(vp[1], vp[0]), rb.Vector2i(vp[3], vp[2]))
         shapes = []
-        for v, i, uv, n, uvi, ni, col, mid, lid in shape_args:
-            assert v.is_contiguous() and i.is_contiguous()
-            shapes.append(rb.Shape(fp(v), ip(i), fp(uv), fp(n), ip(uvi), ip(ni), fp(col), int(v.shape[0]), int(uv.shape[0]) if uv is not None else 0,
-                                   int(n.shape[0]) if n is not None else 0, int(i.shape[0]), mid, lid))
-
-        def make_tex(cls, t, nch_default):
-            if t is None:
-                return cls([], [], [], nch_default, rb.float_ptr(0))
-            mips, uv_scale = t
-            if mips[0].dim() == 3:
-                return cls([fp(m) for m in mips], [int(m.shape[1]) for m in mips], [int(m.shape[0]) for m in mips], int(mips[0].shape[2]), fp(uv_scale))
-            return cls([fp(mips[0])], [0], [0], int(mips[0].shape[0]), fp(uv_scale))
-
+        for s in c.shape_args:
+            assert s.vertices.is_contiguous() and s.indices.is_contiguous()
+            shapes.append(rb.Shape(fp(s.vertices), ip(s.indices), fp(s.uvs), fp(s.normals), ip(s.uv_indices), ip(s.normal_indices), fp(s.colors),
+                                   int(s.vertices.shape[0]), int(s.uvs.shape[0]) if s.uvs is not None else 0,
+                                   int(s.normals.shape[0]) if s.normals is not None else 0, int(s.indices.shape[0]), s.material_id, s.light_id))
         materials = []
-        for texs, spec, two_sided, vcol in mat_args:
-            materials.append(rb.Material(make_tex(rb.Texture3, texs[0], 3), make_tex(rb.Texture3, texs[1], 3), make_tex(rb.Texture1, texs[2], 1),
-                                         make_tex(rb.TextureN, texs[3], 0), make_tex(rb.Texture3, texs[4], 3), spec, two_sided, vcol))
-        lights = [rb.AreaLight(sid, fp(inten), ts, dv) for sid, inten, ts, dv in light_args]
-        use_gpu = device.type == "cuda"
-        gpu_index = device.index if device.index is not None else -1
+        for m in c.mat_args:
+            textures = [_native_texture(rb, cls, nch, t) for (cls, nch), t in zip(_material_textures(rb), m.textures)]
+            materials.append(rb.Material(*textures, m.compute_specular_lighting, m.two_sided, m.use_vertex_color))
+        lights = [rb.AreaLight(l.shape_id, fp(l.intensity), l.two_sided, l.directly_visible) for l in c.light_args]
         envmap = None
-        if env_args is not None:
-            mips, uv_scale, e2w, w2e, cdf_ys, cdf_xs, pdf_norm, visible = env_args
-            env_tex = rb.Texture3([fp(m) for m in mips], [int(m.shape[1]) for m in mips], [int(m.shape[0]) for m in mips], 3, fp(uv_scale))
-            envmap = rb.EnvironmentMap(env_tex, fp(e2w), fp(w2e), fp(cdf_ys), fp(cdf_xs), pdf_norm, visible)
-        c.env_args, c.envmap, c.pixel_filter = env_args, envmap, pixel_filter
+        if c.env_args is not None:
+            e = c.env_args
+            env_tex = _native_texture(rb, rb.Texture3, 3, e.values)
+            envmap = rb.EnvironmentMap(env_tex, fp(e.env_to_world), fp(e.world_to_env), fp(e.sample_cdf_ys), fp(e.sample_cdf_xs), e.pdf_norm,
+                                       e.directly_visible)
+        c.envmap, c.pixel_filter = envmap, opt.pixel_filter
         if scene is None:
             # (the keyword only when a filter is set: a backend without pixel filters renders the 1-pixel box)
-            c.scene = rb.Scene(camera, shapes, materials, lights, envmap, use_gpu, gpu_index, use_prim, use_sec,
-                               **({} if pixel_filter is None else {"pixel_filter": pixel_filter}))
+            c.scene = rb.Scene(camera, shapes, materials, lights, envmap, device.type == "cuda", device.index if device.index is not None else -1,
+                               opt.use_primary_edge_sampling, opt.use_secondary_edge_sampling,
+                               **({} if opt.pixel_filter is None else {"pixel_filter": opt.pixel_filter}))
         elif geometry_changed is not None:
-            scene.update(camera, shapes, materials, lights, envmap, geometry_changed=geometry_changed, pixel_filter=pixel_filter)
+            scene.update(camera, shapes, materials, lights, envmap, geometry_changed=geometry_changed, pixel_filter=opt.pixel_filter)
             c.scene = scene
         else:
             scene.set_camera(camera)
             c.scene = scene
-        ns = num_samples if isinstance(num_samples, (tuple, list)) else (num_samples, num_samples)
-        channels = [rb.channels(int(ch)) for ch in channels]
-        c.options = rb.RenderOptions(seed[0], ns[0], max_bounces, channels, rb.SamplerType(int(sampler_type)), pixel_center)
+        ns = opt.num_samples if isinstance(opt.num_samples, (tuple, list)) else (opt.num_samples, opt.num_samples)
+        channels = [rb.channels(int(ch)) for ch in opt.channels]
+        c.options = rb.RenderOptions(seed[0], ns[0], opt.max_bounces, channels, rb.SamplerType(int(opt.sampler_type)), opt.sample_pixel_center)
         c.camera, c.shapes, c.materials, c.lights = camera, shapes, materials, lights
-        c.shape_args, c.mat_args, c.light_args = shape_args, mat_args, light_args
-        c.num_samples, c.channels, c.viewport, c.device, c.backend, c.seed = ns, channels, viewport, device, rb, seed
-        c.use_look_at = c2w is None
-        c.has_distortion = dist is not None
+        c.num_samples, c.channels, c.viewport, c.device, c.backend, c.seed = ns, channels, vp, device, rb, seed
         return c
 
     @staticmethod
     def forward(ctx, seed, *args):
-        assert isinstance(seed, (tuple, int))
-        if not isinstance(seed, tuple):
-            seed = (seed, seed if _use_correlated_random_number else seed + 1000003)
-        c = RenderFunction._unpack(seed, args)
-        rb = c.backend
-        nch = rb.compute_num_channels(c.channels, c.scene.max_generic_texture_dimension)
-        h, w = c.viewport[2] - c.viewport[0], c.viewport[3] - c.viewport[1]
-        img = torch.zeros(h, w, nch, device=c.device)
-        rb.render(c.scene, c.options, rb.float_ptr(img.data_ptr()), rb.float_ptr(0), None, rb.float_ptr(0), rb.float_ptr(0))
+        c = RenderFunction._unpack(_seeds(seed), args)
         ctx.c = c
         ctx.args = args  # keeps the tensors alive (the native side only holds raw pointers)
-        return img
+        return _render(c)
 
     @staticmethod
     def gradient_buffers(c, zeros=None):
-        """Zeroed gradient buffers for every differentiable input of the unpacked call `c`, and the DScene that points at them (`.d_scene`).
-        `zeros(*shape)` allocates one buffer (default: torch.zeros on c.device)."""
-        rb, dev = c.backend, c.device
+        """Zeroed gradient buffers for every differentiable input of `c` (the unpacked call, or read_args' result alone), and the DScene
+        that points at them (`.d_scene`).  `zeros(*shape)` allocates one buffer (default: torch.zeros on the render device).
+
+        The buffers, in the order they are allocated: `camera` (the eight of rb.DCamera, None where there is none), `shapes` ((vertices,
+        uvs, normals, colors) per shape), `materials` (per material its five textures, each None or (mips, uv_scale)), `intensities` (per
+        light) and `envmap` (None or (mips, uv_scale, world_to_env)).  `grads` maps the position in serialize_scene's list of each argument
+        that has a buffer to that buffer."""
+        rb, dev, p = c.option_args.backend, c.option_args.device, c.pos
         z = zeros or (lambda *shape: torch.zeros(*shape, device=dev))
         fp = lambda t: _ptr(rb, t, "float")  # noqa: E731
-        g = _Ctx()
-        if c.use_look_at:
-            d_pos, d_look, d_up, d_c2w, d_w2c = z(3), z(3), z(3), None, None
-        else:
-            d_pos, d_look, d_up, d_c2w, d_w2c = None, None, None, z(4, 4), z(4, 4)
-        d_intr_inv, d_intr = z(3, 3), z(3, 3)
-        d_dist = z(8) if c.has_distortion else None
-        g.camera = (d_pos, d_look, d_up, d_c2w, d_w2c, d_intr_inv, d_intr, d_dist)
-        d_camera = rb.DCamera(*[fp(t) for t in g.camera])
-        g.shapes, d_shapes = [], []
-        for v, i, uv, n, uvi, ni, col, mid, lid in c.shape_args:
-            bufs = (z(*v.shape), z(*uv.shape) if uv is not None else None, z(*n.shape) if n is not None else None, z(*col.shape) if col is not None else None)
-            g.shapes.append(bufs)
-            d_shapes.append(rb.DShape(fp(bufs[0]), fp(bufs[1]), fp(bufs[2]), fp(bufs[3])))
+        g = SimpleNamespace(grads={})
 
-        def make_dtex(cls, t, nch_default):
-            if t is None:
-                return None, cls([], [], [], nch_default, rb.float_ptr(0))
-            mips, uv_scale = t
-            d_mips = [z(*m.shape) for m in mips]
-            d_uv = z(2)
-            if mips[0].dim() == 3:
-                tex = cls([fp(m) for m in d_mips], [int(m.shape[1]) for m in mips], [int(m.shape[0]) for m in mips], int(mips[0].shape[2]), fp(d_uv))
-            else:
-                tex = cls([fp(d_mips[0])], [0], [0], int(mips[0].shape[0]), fp(d_uv))
-            return (d_mips, d_uv), tex
+        def buf(pos, *shape):
+            g.grads[pos] = z(*shape)
+            return g.grads[pos]
 
-        g.materials, d_materials = [], []
-        for texs, spec, two_sided, vcol in c.mat_args:
-            classes = (rb.Texture3, rb.Texture3, rb.Texture1, rb.TextureN, rb.Texture3)
-            made = [make_dtex(cls, t, nd) for cls, t, nd in zip(classes, texs, (3, 3, 1, 0, 3))]
-            g.materials.append([m[0] for m in made])
-            d_materials.append(rb.DMaterial(*[m[1] for m in made]))
-        g.intensities = [z(3) for _ in c.light_args]
-        d_lights = [rb.DAreaLight(fp(t)) for t in g.intensities]
-        d_envmap, g.envmap = None, None
+        def like(t, pos):  # (None for an absent optional tensor)
+            return buf(pos, *t.shape) if t is not None else None
+
+        def texture(t, pos):
+            return ([buf(q, *m.shape) for q, m in zip(pos.mips, t.mips)], buf(pos.uv_scale, 2)) if t is not None else None
+
+        cam, cp = c.camera_args, p.camera_args
+        look_at = cam.cam_to_world is None  # (which pose the native camera uses: _unpack)
+        g.camera = (buf(cp.position, 3) if look_at else None, buf(cp.look_at, 3) if look_at else None, buf(cp.up, 3) if look_at else None,
+                    None if look_at else buf(cp.cam_to_world, 4, 4), None if look_at else buf(cp.world_to_cam, 4, 4),
+                    buf(cp.intrinsic_mat_inv, 3, 3), buf(cp.intrinsic_mat, 3, 3),
+                    buf(cp.distortion_params, 8) if cam.distortion_params is not None else None)
+        g.shapes = [(like(s.vertices, q.vertices), like(s.uvs, q.uvs), like(s.normals, q.normals), like(s.colors, q.colors))
+                    for s, q in zip(c.shape_args, p.shape_args)]
+        g.materials = [[texture(t, q) for t, q in zip(m.textures, mp.textures)] for m, mp in zip(c.mat_args, p.mat_args)]
+        g.intensities = [buf(q.intensity, 3) for q in p.light_args]
+        g.envmap = d_envmap = None
         if c.env_args is not None:  # pyredner/render_pytorch.py:948-968
-            mips = c.env_args[0]
-            g.envmap = ([z(*m.shape) for m in mips], z(2), z(4, 4))
-            d_env_tex = rb.Texture3([fp(m) for m in g.envmap[0]], [int(m.shape[1]) for m in mips], [int(m.shape[0]) for m in mips], 3, fp(g.envmap[1]))
-            d_envmap = rb.DEnvironmentMap(d_env_tex, fp(g.envmap[2]))
-        g.d_scene = rb.DScene(d_camera, d_shapes, d_materials, d_lights, d_envmap, dev.type == "cuda", dev.index if dev.index is not None else -1)
+            values = c.env_args.values
+            g.envmap = texture(values, p.env_args.values) + (buf(p.env_args.world_to_env, 4, 4),)
+            d_envmap = rb.DEnvironmentMap(_native_texture(rb, rb.Texture3, 3, values, g.envmap[:2]), fp(g.envmap[2]))
+        d_materials = [rb.DMaterial(*[_native_texture(rb, cls, nch, t, b) for (cls, nch), t, b in zip(_material_textures(rb), m.textures, bufs)])
+                       for m, bufs in zip(c.mat_args, g.materials)]
+        g.d_scene = rb.DScene(rb.DCamera(*[fp(t) for t in g.camera]), [rb.DShape(*[fp(t) for t in b]) for b in g.shapes], d_materials,
+                              [rb.DAreaLight(fp(t)) for t in g.intensities], d_envmap, dev.type == "cuda", dev.index if dev.index is not None else -1)
         return g
 
     @staticmethod
@@ -455,43 +519,16 @@ class RenderFunction(torch.autograd.Function):
 
     @staticmethod
     def gradient_outputs(c, g):
-        """backward's return value: the buffers of gradient_buffers(c) at the positions of serialize_scene's arguments."""
-        out = [None]  # seed
-        out += [None, None, None]  # counts
-        cpu = lambda t: t.cpu() if t is not None else None  # noqa: E731
-        out += [cpu(t) for t in g.camera]
-        out += [None, None, None, None]  # clip_near, resolution, viewport, camera_type
-        for bufs in g.shapes:
-            out += [bufs[0], None, bufs[1], bufs[2], None, None, bufs[3], None, None]
-        for mb, (texs, _, _, _) in zip(g.materials, c.mat_args):
-            for b, t in zip(mb, texs):
-                out.append(None)  # number of levels
-                if t is not None:
-                    out += list(b[0])
-                    out.append(b[1])
-            out += [None, None, None]
-        for d_i in g.intensities:
-            out += [None, d_i.cpu(), None, None]
-        if g.envmap is not None:  # pyredner/render_pytorch.py:1154-1164
-            out.append(None)  # number of levels
-            out += list(g.envmap[0])
-            out += [g.envmap[1], None, g.envmap[2].cpu(), None, None, None, None]  # uv_scale, env_to_world, world_to_env, cdfs, pdf_norm, visible
-        else:
-            out.append(None)  # envmap
-        out += [None] * 10  # num_samples .. backend
+        """backward's return value: None for the seed, then the buffers of gradient_buffers(c) at the positions of serialize_scene's
+        arguments, each on the device of its argument (the host for the camera, the light intensities and world_to_env)."""
+        out = [None] * (1 + len(c.args))
+        for pos, t in g.grads.items():
+            out[1 + pos] = t.to(c.args[pos].device)
         return tuple(out)
 
     @staticmethod
     def backward(ctx, grad_img):
-        c = ctx.c
-        rb = c.backend
-        if not grad_img.is_contiguous():
-            grad_img = grad_img.contiguous()
-        assert torch.isfinite(grad_img).all()
-        g = RenderFunction.gradient_buffers(c)
-        screen_grad = getattr(c, "screen_gradient", None)  # (only set by visualize_screen_gradient)
-        rb.render(c.scene, RenderFunction.backward_options(c), rb.float_ptr(0), _ptr(rb, grad_img), g.d_scene, _ptr(rb, screen_grad), rb.float_ptr(0))
-        return RenderFunction.gradient_outputs(c, g)
+        return _backward(ctx.c, grad_img)
 
 
 class BatchRenderFunction(torch.autograd.Function):
@@ -510,14 +547,9 @@ class BatchRenderFunction(torch.autograd.Function):
             sd = seeds[k] if isinstance(seeds[k], tuple) else (seeds[k], seeds[k] + 1000003)
             c = RenderFunction._unpack(sd, args[k * n:(k + 1) * n], scene=scene)
             scene = c.scene
-            rb = c.backend
-            nch = rb.compute_num_channels(c.channels, c.scene.max_generic_texture_dimension)
-            h, w = c.viewport[2] - c.viewport[0], c.viewport[3] - c.viewport[1]
-            img = torch.zeros(h, w, nch, device=c.device)
-            rb.render(c.scene, c.options, rb.float_ptr(img.data_ptr()), rb.float_ptr(0), None, rb.float_ptr(0), rb.float_ptr(0))
             views.append(c)
-            imgs.append(img)
-        ctx.views, ctx.args, ctx.n = views, args, n
+            imgs.append(_render(c))
+        ctx.views, ctx.args = views, args
         return torch.stack(imgs)
 
     @staticmethod
@@ -525,9 +557,7 @@ class BatchRenderFunction(torch.autograd.Function):
         out = [None, None]
         for k, c in enumerate(ctx.views):
             c.scene.set_camera(c.camera)
-            one = _Ctx()
-            one.c, one.args = c, ctx.args[k * ctx.n:(k + 1) * ctx.n]
-            out += list(RenderFunction.backward(one, grad_imgs[k]))[1:]
+            out += _backward(c, grad_imgs[k])[1:]
         return tuple(out)
 
 
@@ -554,43 +584,28 @@ class SceneRenderer:
         self._indices = None     # [(index tensor, its _version, copy)] of the build
 
     @staticmethod
-    def _structure(args):
-        """The parts of a serialize_scene list that rb_scene_update requires to be unchanged, except the contents of index buffers."""
-        it = iter(args)
-        nxt = lambda: next(it)  # noqa: E731
-        num_shapes, num_materials, num_lights = nxt(), nxt(), nxt()
-        for _ in range(12):
-            nxt()
-        shapes, mats, lights = [], [], []
-        for _ in range(num_shapes):
-            v, i, uv, n, uvi, ni, col, mid, lid = [nxt() for _ in range(9)]
-            shapes.append((tuple(v.shape), tuple(i.shape), tuple(uv.shape) if uv is not None else None, tuple(n.shape) if n is not None else None,
-                           uvi is not None, ni is not None, col is not None, int(mid), int(lid)))
-        for _ in range(num_materials):
-            texs = []
-            for _ in range(5):
-                k = nxt()
-                texs.append(None if k == 0 else tuple(tuple(nxt().shape) for _ in range(k + 1)))  # (mip levels, then uv_scale)
-            mats.append((tuple(texs), nxt(), nxt(), nxt()))
-        for _ in range(num_lights):
-            lights.append(int(nxt()))
-            nxt(), nxt(), nxt()
-        k = nxt()
-        env = None if k is None else tuple(tuple(nxt().shape) for _ in range(k + 1))  # (mip levels, then uv_scale)
-        if k is not None:
-            for _ in range(6):  # matrices, sampling tables, pdf_norm, directly_visible
-                nxt()
-        rest = [nxt() for _ in range(10)]
-        flags = (bool(rest[4]), bool(rest[5]), str(rest[8]))  # edge-sampling flags, device
-        return tuple(shapes), tuple(mats), tuple(lights), env, flags
+    def _structure(a):
+        """The parts of a read_args result that rb_scene_update requires to be unchanged, except the contents of index buffers."""
+        def shape(t):
+            return tuple(t.shape) if t is not None else None
+
+        def texture(t):
+            return None if t is None else tuple(shape(m) for m in t.mips) + (shape(t.uv_scale),)
+        shapes = tuple((shape(s.vertices), shape(s.indices), shape(s.uvs), shape(s.normals), s.uv_indices is not None, s.normal_indices is not None,
+                        s.colors is not None, int(s.material_id), int(s.light_id)) for s in a.shape_args)
+        mats = tuple((tuple(texture(t) for t in m.textures), m.compute_specular_lighting, m.two_sided, m.use_vertex_color) for m in a.mat_args)
+        lights = tuple(int(l.shape_id) for l in a.light_args)
+        env = texture(a.env_args.values) if a.env_args is not None else None
+        o = a.option_args
+        return shapes, mats, lights, env, (bool(o.use_primary_edge_sampling), bool(o.use_secondary_edge_sampling), str(o.device))
 
     def _target(self, args):
         """(geometry_changed, state): geometry_changed is None to build a new native scene for `args`, else the flag for an update of the
         current one; `state` is what _commit records once the native call has succeeded."""
-        key = self._structure(args)
-        n = args[0]
-        verts = [args[15 + 9 * s] for s in range(n)]
-        inds = [args[16 + 9 * s] for s in range(n)]
+        a = RenderFunction.read_args(args)
+        key = self._structure(a)
+        verts = [s.vertices for s in a.shape_args]
+        inds = [s.indices for s in a.shape_args]
         fresh = self._scene is None or key != self._key
         if not fresh:
             for t, (t0, ver0, copy) in zip(inds, self._indices):
@@ -621,9 +636,7 @@ class SceneRenderer:
 class _SceneRenderFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, seed, renderer, *args):
-        assert isinstance(seed, (tuple, int))
-        if not isinstance(seed, tuple):
-            seed = (seed, seed if _use_correlated_random_number else seed + 1000003)
+        seed = _seeds(seed)
         geometry, state = renderer._target(args)
         try:
             c = RenderFunction._unpack(seed, args, scene=renderer._scene if geometry is not None else None, geometry_changed=geometry)
@@ -633,14 +646,9 @@ class _SceneRenderFunction(torch.autograd.Function):
         renderer._commit(c.scene, state)
         c.scene._generation = getattr(c.scene, "_generation", 0) + 1
         ctx.generation = c.scene._generation
-        rb = c.backend
-        nch = rb.compute_num_channels(c.channels, c.scene.max_generic_texture_dimension)
-        h, w = c.viewport[2] - c.viewport[0], c.viewport[3] - c.viewport[1]
-        img = torch.zeros(h, w, nch, device=c.device)
-        rb.render(c.scene, c.options, rb.float_ptr(img.data_ptr()), rb.float_ptr(0), None, rb.float_ptr(0), rb.float_ptr(0))
         ctx.c = c
         ctx.args = args  # keeps the tensors alive (the native side only holds raw pointers)
-        return img
+        return _render(c)
 
     @staticmethod
     def backward(ctx, grad_img):
@@ -649,7 +657,7 @@ class _SceneRenderFunction(torch.autograd.Function):
             c.scene.update(c.camera, c.shapes, c.materials, c.lights, c.envmap, geometry_changed=True, pixel_filter=c.pixel_filter)
             c.scene._generation += 1
             ctx.generation = c.scene._generation
-        return (None,) + RenderFunction.backward(ctx, grad_img)
+        return (None,) + _backward(c, grad_img)
 
 
 def render_batch(scenes, num_samples, max_bounces: int, seeds, **kw) -> torch.Tensor:
@@ -671,17 +679,13 @@ def visualize_screen_gradient(grad_img: Optional[torch.Tensor], seed: int, scene
                                           sample_pixel_center=sample_pixel_center, device=device, backend=backend)
     c = RenderFunction._unpack((seed, seed), args)
     c.num_samples = (c.num_samples[0], c.num_samples[0])  # (the reference renders this pass with the forward sample count)
-    rb = c.backend
-    nch = rb.compute_num_channels(c.channels, c.scene.max_generic_texture_dimension)
-    h, w = c.viewport[2] - c.viewport[0], c.viewport[3] - c.viewport[1]
+    h, w, nch = _image_shape(c)
     if grad_img is None:
         grad_img = torch.ones(h, w, nch, device=c.device)
     assert tuple(grad_img.shape) == (h, w, nch)
-    c.screen_gradient = torch.zeros(h, w, 2, device=c.device)
-    ctx = _Ctx()
-    ctx.c, ctx.args = c, args
-    RenderFunction.backward(ctx, grad_img.to(c.device))
-    return c.screen_gradient
+    screen_grad = torch.zeros(h, w, 2, device=c.device)
+    _backward(c, grad_img.to(c.device), screen_grad)
+    return screen_grad
 
 
 RenderFunction.visualize_screen_gradient = staticmethod(visualize_screen_gradient)  # (where pyredner keeps it)

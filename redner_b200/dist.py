@@ -84,12 +84,8 @@ class TileRenderFunction(torch.autograd.Function):
         if not isinstance(seed, tuple):
             seed = (seed, seed + 1000003)
         c = api.RenderFunction._unpack(seed, args)
-        rb = c.backend
         c.scene.set_partition(rank, world, rows_per_stripe)
-        nch = rb.compute_num_channels(c.channels, c.scene.max_generic_texture_dimension)
-        h, w = c.viewport[2] - c.viewport[0], c.viewport[3] - c.viewport[1]
-        img = torch.zeros(h, w, nch, device=c.device)
-        rb.render(c.scene, c.options, rb.float_ptr(img.data_ptr()), rb.float_ptr(0), None, rb.float_ptr(0), rb.float_ptr(0))
+        img = api._render(c)
         dist.all_reduce(img, op=dist.ReduceOp.SUM, group=group)  # disjoint stripes: a sum is a gather
         ctx.c, ctx.args, ctx.group = c, args, group
         return img
@@ -101,21 +97,9 @@ class TileRenderFunction(torch.autograd.Function):
             grad_img = grad_img.contiguous()
             assert torch.isfinite(grad_img).all()
             return (None, None, None) + _exact_backward(ctx.c, grad_img, ctx.group)[1:]
-        ctx_like = type("C", (), {})()
-        ctx_like.c, ctx_like.args = ctx.c, ctx.args
-        grads = api.RenderFunction.backward(ctx_like, grad_img)
-        tens = [g for g in grads if isinstance(g, torch.Tensor)]
-        dev = ctx.c.device
-        moved = [t.to(dev) for t in tens]
-        reduced = all_reduce_packed(moved, ctx.group)
-        it = iter(reduced)
-        out = []
-        for g in grads:
-            if isinstance(g, torch.Tensor):
-                r = next(it)
-                out.append(r.to(g.device))
-            else:
-                out.append(g)
+        grads = api._backward(ctx.c, grad_img)
+        reduced = iter(all_reduce_packed([g.to(ctx.c.device) for g in grads if isinstance(g, torch.Tensor)], ctx.group))
+        out = [next(reduced).to(g.device) if isinstance(g, torch.Tensor) else g for g in grads]
         return (None, None, None) + tuple(out[1:])
 
 

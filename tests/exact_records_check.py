@@ -56,20 +56,8 @@ def prepare(rb, dev, cfg, kind):
 
 
 def buffers(c, g, screen):
-    """Every gradient buffer of gradient_buffers(c) (the camera's included) and the screen-gradient image, flattened, in a fixed order."""
-    out = [t for t in g.camera if t is not None]
-    for bufs in g.shapes:
-        out += [t for t in bufs if t is not None]
-    for mb in g.materials:
-        for b in mb:
-            if b is not None:
-                out += list(b[0]) + [b[1]]
-    out += list(g.intensities)
-    if g.envmap is not None:
-        out += list(g.envmap[0]) + [g.envmap[1], g.envmap[2]]
-    if screen is not None:
-        out.append(screen)
-    return out
+    """Every gradient buffer of gradient_buffers(c) (the camera's included) and the screen-gradient image, in a fixed order."""
+    return list(g.grads.values()) + ([screen] if screen is not None else [])
 
 
 def carve(c, with_screen, reverse):

@@ -213,26 +213,11 @@ def test_render_batch_equals_the_sequence_of_renders(rb, dev, deterministic):
     def descriptor(c):
         """A gradient descriptor of the scene with zeroed buffers (the layout RenderFunction.backward makes) and the buffers."""
         keep = []
-        fp = lambda t: api._ptr(rb, t, "float")  # noqa: E731
 
-        def buf(*shape):
+        def zeros(*shape):
             keep.append(torch.zeros(*shape, device=dev))
-            return fp(keep[-1])
-
-        def dtex(cls, t, nd):
-            if t is None:
-                return cls([], [], [], nd, rb.float_ptr(0))
-            mips = t[0]
-            if mips[0].dim() == 3:
-                return cls([buf(*m.shape) for m in mips], [int(m.shape[1]) for m in mips], [int(m.shape[0]) for m in mips], int(mips[0].shape[2]), buf(2))
-            return cls([buf(*mips[0].shape)], [0], [0], int(mips[0].shape[0]), buf(2))
-        d_camera = rb.DCamera(buf(3), buf(3), buf(3), fp(None), fp(None), buf(3, 3), buf(3, 3), fp(None))
-        d_shapes = [rb.DShape(buf(*v.shape), buf(*uv.shape) if uv is not None else fp(None), buf(*n.shape) if n is not None else fp(None),
-                              buf(*col.shape) if col is not None else fp(None)) for v, _, uv, n, _, _, col, _, _ in c.shape_args]
-        classes = (rb.Texture3, rb.Texture3, rb.Texture1, rb.TextureN, rb.Texture3)
-        d_mats = [rb.DMaterial(*[dtex(cls, t, nd) for cls, t, nd in zip(classes, texs, (3, 3, 1, 0, 3))]) for texs, _, _, _ in c.mat_args]
-        d_lights = [rb.DAreaLight(buf(3)) for _ in c.light_args]
-        return rb.DScene(d_camera, d_shapes, d_mats, d_lights, None, True, dev.index or 0), keep
+            return keep[-1]
+        return api.RenderFunction.gradient_buffers(c, zeros).d_scene, keep
 
     def options(c):
         o = L.rb_options(seed=c.seed[1], num_samples=c.num_samples[1], max_bounces=c.options.max_bounces, sampler_type=int(c.options.sampler_type),
