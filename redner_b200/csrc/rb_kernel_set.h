@@ -1,6 +1,7 @@
 // The render kernels that exist in every instantiation of rb_kernels_body.cuh, as host-side kernel pointers for
 // cudaLaunchKernel: ::render_kernels() returns the general set (rb_kernels.cu), rb_lean::render_kernels() the feature-free
-// set (rb_kernels_lean.cu), rb_det::render_kernels() the general set with the deterministic gradient scatter (rb_kernels_det.cu).
+// set (rb_kernels_lean.cu), rb_diffuse::render_kernels() the feature-free set for diffuse-only materials (rb_kernels_diffuse.cu),
+// rb_det::render_kernels() the general set with the deterministic gradient scatter (rb_kernels_det.cu).
 // All sets take the same arguments: the other translation units declare the same DevScene / KernelArgs layouts inside their
 // namespaces, so the driver's structs are passed to any of them as they are.
 #pragma once
@@ -9,6 +10,9 @@ struct RenderKernels {
 };
 RenderKernels render_kernels();
 namespace rb_lean {
+RenderKernels render_kernels();
+}
+namespace rb_diffuse {
 RenderKernels render_kernels();
 }
 namespace rb_det {

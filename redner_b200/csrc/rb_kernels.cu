@@ -129,13 +129,17 @@ static int render_pass(const rb_scene* scene_, const rb_options* opt, float* ima
     }
     const RenderParams& rp = ka.rp;
     if (rp.vp_w <= 0 || rp.vp_h <= 0 || rp.spp == 0) return 0;
-    // The feature-free instantiation of the kernels (rb_kernels_lean.cu) serves the common configuration; `kern` holds the kernels of
-    // the chosen instantiation, and every launch of one of them below goes through it.
-    const bool lean_allowed = getenv("RB_NO_LEAN") == nullptr; // (test hook: force the general kernels)
+    // The feature-free instantiation of the kernels (rb_kernels_lean.cu) serves the common configuration, and its diffuse-only refinement
+    // (rb_kernels_diffuse.cu) the scenes of that configuration whose materials are all diffuse; `kern` holds the kernels of the chosen
+    // instantiation, and every launch of one of them below goes through it.  The materials are read from the scene's host copies on every
+    // call: rb_scene_update may have changed their flags.
+    const bool lean_allowed = getenv("RB_NO_LEAN") == nullptr;       // (test hook: force the general kernels)
+    const bool diffuse_allowed = getenv("RB_NO_DIFFUSE") == nullptr; // (test hook: force the lean kernels where the diffuse ones would run)
     const DevCamera& cam = scene->dev.cam;
     const bool lean = lean_allowed && rp.only_radiance && !scene->dev.has_envmap && cam.type == RB_CAMERA_PERSPECTIVE && !cam.has_distortion &&
                       cam.filter_type == RB_FILTER_BOX && cam.filter_width == 1.0f;
-    const RenderKernels kern = lean ? rb_lean::render_kernels() : render_kernels();
+    const bool diffuse = lean && diffuse_allowed && materials_diffuse_only(scene->materials.data(), (int)scene->materials.size());
+    const RenderKernels kern = diffuse ? rb_diffuse::render_kernels() : lean ? rb_lean::render_kernels() : render_kernels();
     // Deterministic mode: the backward kernels of rb_kernels_det.cu (the forward kernels are deterministic as they are).  Records
     // come from the exact accumulators, so rb_render_exact runs them whatever the options say.
     const bool det = opt->deterministic != 0 || xo != nullptr;

@@ -185,7 +185,14 @@ RB_HD V3 mat_diffuse(const rb_material& m, const SurfacePoint& p) { return tex_e
 RB_HD V3 mat_specular(const rb_material& m, const SurfacePoint& p) { return tex_eval(m.specular_reflectance, 3, p.uv, p.du_dxy, p.dv_dxy); }
 RB_HD Real mat_roughness(const rb_material& m, const SurfacePoint& p) { return tex_eval(m.roughness, 1, p.uv, p.du_dxy, p.dv_dxy).x; }
 RB_HD V3 mat_normal_tex(const rb_material& m, const SurfacePoint& p) { return tex_eval(m.normal_map, 3, p.uv, p.du_dxy, p.dv_dxy); }
-RB_HD bool mat_has_normal_map(const rb_material& m) { return m.normal_map.num_levels > 0; }
+RB_HD bool mat_has_normal_map(const rb_material& m) { return RB_NORMAL_MAP(m); }
+// True when no material sets a flag that RB_SPECULAR, RB_VERTEX_COLOR or RB_NORMAL_MAP tests, i.e. when the diffuse-only kernels
+// (RB_DIFFUSE, rb_kernels_diffuse.cu) compute what the others do.  Tests the fields themselves, so that it answers the same in every build.
+inline bool materials_diffuse_only(const rb_material* m, int n) {
+    for (int i = 0; i < n; i++)
+        if (m[i].compute_specular_lighting != 0 || m[i].use_vertex_color != 0 || m[i].normal_map.num_levels > 0) return false;
+    return true;
+}
 RB_HD Real roughness_to_phong(Real r) { return rb_max(2 / r - 2, Real(0)); }
 RB_HD Real d_roughness_to_phong(Real r, Real d_e) { return (r > 0 && r <= 1) ? -2 * d_e / rb_sq(r) : Real(0); }
 
@@ -227,8 +234,8 @@ struct MatTex {
 };
 RB_HD MatTex mat_textures(const rb_material& m, const SurfacePoint& p) {
     MatTex t;
-    t.kd = max3(m.use_vertex_color ? p.color : mat_diffuse(m, p), 0);
-    t.ks = max3(m.use_vertex_color ? zero3() : mat_specular(m, p), 0);
+    t.kd = max3(RB_VERTEX_COLOR(m) ? p.color : mat_diffuse(m, p), 0);
+    t.ks = max3(RB_VERTEX_COLOR(m) ? zero3() : mat_specular(m, p), 0);
     t.rough = mat_roughness(m, p);
     return t;
 }
@@ -254,7 +261,7 @@ RB_HD V3 bsdf_eval(const rb_material& m, const SurfacePoint& p, const MatTex& tx
     Real roughness = rb_max(tx.rough, min_rough);
     V3 diffuse = kd * (sh_wo / RB_PI);
     V3 spec = zero3();
-    if (m.compute_specular_lighting && !m.use_vertex_color) {
+    if (RB_SPECULAR(m) && !RB_VERTEX_COLOR(m)) {
         V3 h = normalize(wi + wo);
         V3 hl = to_local(c.frame, h);
         if (m.two_sided && hl.z < 0) hl = -hl;
@@ -368,17 +375,17 @@ RB_D void d_bsdf_eval(const rb_material& m, const rb_material& d_m, const Surfac
     const V3 kd = tx.kd, ks = tx.ks;
     // diffuse = kd * sh_wo / pi   (gradient passes through the clamp unchanged, src/material.h:505-518)
     V3 d_kd = d_out * (sh_wo / RB_PI);
-    if (m.use_vertex_color) d_p.color += d_kd;
+    if (RB_VERTEX_COLOR(m)) d_p.color += d_kd;
     // texture adjoints are collected here and scattered by ONE rolled loop at the end (one copy of the mip adjoint)
     V3 d_slot[4] = {d_kd, zero3(), zero3(), zero3()};
-    unsigned slot_on = m.use_vertex_color ? 0u : 1u;
+    unsigned slot_on = RB_VERTEX_COLOR(m) ? 0u : 1u;
     Real d_sh_wo = sum(d_out * kd) / RB_PI;
     if (dot(n, wo) < 0) d_sh_wo = -d_sh_wo;
     d_wo += n * d_sh_wo;
     d_n += wo * d_sh_wo;
 
     Real roughness = rb_max(rb_max(tx.rough, min_rough), Real(1e-6));
-    if (m.compute_specular_lighting && !m.use_vertex_color) {
+    if (RB_SPECULAR(m) && !RB_VERTEX_COLOR(m)) {
         V3 h = normalize(wi + wo);
         V3 hl = to_local(c.frame, h);
         bool flipped = false;

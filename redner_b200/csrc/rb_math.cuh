@@ -47,6 +47,22 @@ typedef float Real;
 #define RB_ONLY_RADIANCE(rp) ((rp).only_radiance != 0)
 #define RB_PIXEL_BOX(cam) ((cam).filter_type == RB_FILTER_BOX && (cam).filter_width == 1.0f)
 #endif
+// Material features.  rb_kernels_diffuse.cu compiles the lean kernels once more with RB_DIFFUSE defined as well: no material
+// computes specular lighting, uses vertex colours or has a normal map -- the diffuse-only scenes of shape and pose optimisation.
+// Only the host-known flags are folded; texel values (the specular reflectance that weights lobe selection included) are read
+// and used as in every other build.
+#ifdef RB_DIFFUSE
+#ifndef RB_LEAN
+#error "RB_DIFFUSE is a refinement of RB_LEAN"
+#endif
+#define RB_SPECULAR(m) false
+#define RB_VERTEX_COLOR(m) false
+#define RB_NORMAL_MAP(m) false
+#else
+#define RB_SPECULAR(m) ((m).compute_specular_lighting != 0)
+#define RB_VERTEX_COLOR(m) ((m).use_vertex_color != 0)
+#define RB_NORMAL_MAP(m) ((m).normal_map.num_levels > 0)
+#endif
 
 #ifndef M_PI
 #define M_PI 3.14159265358979323846

@@ -260,7 +260,7 @@ RB_D void channel_values_at_hit(const DevScene& sc, const RenderParams& rp, cons
             case RB_CH_UV: vals[d] = sp.uv.x; vals[d + 1] = sp.uv.y; d += 2; break;
             case RB_CH_BARYCENTRIC: vals[d] = sp.bary.x; vals[d + 1] = sp.bary.y; d += 2; break;
             case RB_CH_DIFFUSE_REFLECTANCE: {
-                V3 r = mat.use_vertex_color ? sp.color : mat_diffuse(mat, sp);
+                V3 r = RB_VERTEX_COLOR(mat) ? sp.color : mat_diffuse(mat, sp);
                 vals[d] = r.x; vals[d + 1] = r.y; vals[d + 2] = r.z;
                 d += 3;
             } break;
@@ -310,7 +310,7 @@ RB_D void d_channel_values_at_hit(const DevScene& sc, const DevDScene& ds, const
             case RB_CH_UV: d_sp.uv += mk2(d_vals[d], d_vals[d + 1]); d += 2; break;
             case RB_CH_BARYCENTRIC: d_sp.bary += mk2(d_vals[d], d_vals[d + 1]); d += 2; break;
             case RB_CH_DIFFUSE_REFLECTANCE:
-                if (mat.use_vertex_color) d_sp.color += mk3(d_vals[d], d_vals[d + 1], d_vals[d + 2]);
+                if (RB_VERTEX_COLOR(mat)) d_sp.color += mk3(d_vals[d], d_vals[d + 1], d_vals[d + 2]);
                 else d_tex_eval(mat.diffuse_reflectance, d_mat.diffuse_reflectance, 3, sp.uv, sp.du_dxy, sp.dv_dxy, d_vals + d, d_sp.uv, d_sp.du_dxy, d_sp.dv_dxy);
                 d += 3;
                 break;

@@ -389,6 +389,13 @@ static int emu_render(const rb_scene* scene, const rb_options* opt, float* image
     }
     const RenderParams& rp = ka.rp;
     if (rp.vp_w <= 0 || rp.vp_h <= 0 || rp.spp == 0) return 0;
+#ifdef RB_DIFFUSE
+    // the library runs its diffuse-only kernels only for such materials (rb_kernels.cu); this build computes nothing else correctly
+    if (!materials_diffuse_only(scene->materials.data(), (int)scene->materials.size())) {
+        g_err = "rb_render: this build serves diffuse-only materials (no specular lighting, vertex colours or normal map)";
+        return 1;
+    }
+#endif
     const DevScene& sc = scene->dev;
     if (image && !rp.only_radiance) {
         for (int j = 0; j < ka.owned_rows; j++)

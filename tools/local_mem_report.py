@@ -2,8 +2,9 @@
 """Local-memory report of the render kernels: registers, stack frame, spills and the static LDL / STL instructions of every hot
 kernel, with the source lines they come from.  Needs nvcc and nvdisasm, no GPU.
 
-    python tools/local_mem_report.py                     # the lean instantiation (the one C2, C3 and C4 run)
-    python tools/local_mem_report.py --tu lean general det --top 8
+    python tools/local_mem_report.py                     # the lean instantiation (the one C3 and C4 run)
+    python tools/local_mem_report.py --tu diffuse        # its diffuse-only refinement (the one C2 runs)
+    python tools/local_mem_report.py --tu lean diffuse general det --top 8
     python tools/local_mem_report.py --root OTHER_CHECKOUT   # the same report for another tree (before / after)
 
 Each translation unit is compiled to a cubin with the flags of redner_b200/build.py plus -Xptxas -v, and the cubin is disassembled
@@ -20,7 +21,7 @@ import sys
 import tempfile
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-TUS = {"lean": "rb_kernels_lean.cu", "general": "rb_kernels.cu", "det": "rb_kernels_det.cu"}
+TUS = {"lean": "rb_kernels_lean.cu", "diffuse": "rb_kernels_diffuse.cu", "general": "rb_kernels.cu", "det": "rb_kernels_det.cu"}
 HOT = ["k_forward", "k_bwd_trace", "k_bwd_sec_pick", "k_bwd_sec_shade", "k_bwd_sweep", "k_primary_edge"]
 TEX_FUNCS = ["bilerp_tap", "bilerp_eval", "tex_level", "tex_eval_mip", "tex_eval", "mat_diffuse", "mat_specular", "mat_roughness",
              "mat_normal_tex"]
