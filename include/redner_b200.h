@@ -81,6 +81,11 @@ typedef struct rb_texture {
     float* uv_scale; /* device pointer to 2 floats (may be NULL when num_levels == 0) */
 } rb_texture;
 
+/* Specular lobe of a material (rb_material::specular_model).  Blinn-Phong is the reference's lobe (a Phong exponent 2 / r - 2 with a
+ * rational fit of the Smith term).  GGX (no reference counterpart) is the Trowbridge-Reitz distribution with alpha = sqrt(r),
+ * height-correlated Smith masking-shadowing and sampling of the visible normals; DESIGN.md section "GGX" defines it. */
+enum rb_specular_model { RB_SPECULAR_BLINN_PHONG = 0, RB_SPECULAR_GGX = 1 };
+
 /* Material -- src/material.h:12-91; DMaterial (src/material.h:93-99) uses the same layout with gradient buffers. */
 typedef struct rb_material {
     rb_texture diffuse_reflectance;  /* 3 channels */
@@ -89,6 +94,9 @@ typedef struct rb_material {
     rb_texture generic_texture;      /* N channels, optional */
     rb_texture normal_map;           /* 3 channels, optional */
     int compute_specular_lighting, two_sided, use_vertex_color;
+    /* rb_specular_model; zero-initialised == Blinn-Phong.  Matters only with compute_specular_lighting and without use_vertex_color.
+     * rb_scene_create and rb_scene_update refuse any other value; rb_dscene_desc::materials ignores the field. */
+    int specular_model;
 } rb_material;
 
 /* AreaLight -- src/area_light.h:8-36 */

@@ -53,11 +53,15 @@ class rb_texture(C.Structure):
     ]
 
 
+# enum rb_specular_model
+RB_SPECULAR_BLINN_PHONG, RB_SPECULAR_GGX = 0, 1
+
+
 class rb_material(C.Structure):
     _fields_ = [
         ("diffuse_reflectance", rb_texture), ("specular_reflectance", rb_texture), ("roughness", rb_texture),
         ("generic_texture", rb_texture), ("normal_map", rb_texture),
-        ("compute_specular_lighting", C.c_int), ("two_sided", C.c_int), ("use_vertex_color", C.c_int),
+        ("compute_specular_lighting", C.c_int), ("two_sided", C.c_int), ("use_vertex_color", C.c_int), ("specular_model", C.c_int),
     ]
 
 

@@ -124,8 +124,15 @@ def _as_texture(x, default=None):
 
 
 class Material:
+    """`specular_model` (redner_b200 extension): the specular lobe, "blinn_phong" (the reference's) or "ggx" (Trowbridge-Reitz with
+    alpha = sqrt(roughness), height-correlated Smith masking and visible-normal sampling; DESIGN.md section "GGX").  It matters only with
+    a specular reflectance and without vertex colours."""
+    SPECULAR_MODELS = ("blinn_phong", "ggx")  # rb_specular_model
+
     def __init__(self, diffuse_reflectance=None, specular_reflectance=None, roughness=None, generic_texture=None, normal_map=None,
-                 two_sided: bool = False, use_vertex_color: bool = False):
+                 two_sided: bool = False, use_vertex_color: bool = False, specular_model: str = "blinn_phong"):
+        if specular_model not in self.SPECULAR_MODELS:
+            raise ValueError("Material: specular_model must be one of %s, not %r" % (", ".join(self.SPECULAR_MODELS), specular_model))
         if diffuse_reflectance is None:
             diffuse_reflectance = torch.zeros(3)
         dev = diffuse_reflectance.texels.device if isinstance(diffuse_reflectance, Texture) else diffuse_reflectance.device
@@ -142,6 +149,7 @@ class Material:
         self.compute_specular_lighting = compute_specular
         self.two_sided = two_sided
         self.use_vertex_color = use_vertex_color
+        self.specular_model = specular_model
 
 
 class Shape:
@@ -214,7 +222,7 @@ _MaterialArgs = namedtuple("_MaterialArgs", "textures compute_specular_lighting 
 _LightArgs = namedtuple("_LightArgs", "shape_id intensity two_sided directly_visible")
 _EnvmapArgs = namedtuple("_EnvmapArgs", "values env_to_world world_to_env sample_cdf_ys sample_cdf_xs pdf_norm directly_visible")
 _OptionArgs = namedtuple("_OptionArgs", "num_samples max_bounces channels sampler_type use_primary_edge_sampling use_secondary_edge_sampling "
-                                        "sample_pixel_center pixel_filter device backend")
+                                        "sample_pixel_center pixel_filter device backend specular_models")
 
 
 def _ptr(backend, t, kind="float"):
@@ -292,7 +300,7 @@ class RenderFunction(torch.autograd.Function):
     """torch.autograd.Function around `redner.render` (pyredner/render_pytorch.py:63-1177).
 
     `RenderFunction.apply(seed, *args)` with `args = RenderFunction.serialize_scene(...)`.  The module implementing the
-    `redner` surface is the LAST serialized argument, so the same host code can drive the product and the oracle."""
+    `redner` surface is a serialized argument (`option_args.backend`), so the same host code can drive the product and the oracle."""
 
     @staticmethod
     def serialize_scene(scene: Scene, num_samples: Union[int, Tuple[int, int]], max_bounces: int, channels=None, sampler_type=None,
@@ -356,6 +364,9 @@ class RenderFunction(torch.autograd.Function):
         args += [num_samples, max_bounces, channels, sampler_type]
         args += [use_primary_edge_sampling and vis, use_secondary_edge_sampling and vis]
         args += [sample_pixel_center, pixel_filter.native() if pixel_filter is not None else None, device, backend]
+        # the materials' rb_specular_model values, None when every one is the default (the last entry, so that no other one moves)
+        models = tuple(Material.SPECULAR_MODELS.index(getattr(m, "specular_model", "blinn_phong")) for m in scene.materials)
+        args.append(models if any(models) else None)
         return args
 
     @staticmethod
@@ -429,9 +440,12 @@ class RenderFunction(torch.autograd.Function):
                                    int(s.vertices.shape[0]), int(s.uvs.shape[0]) if s.uvs is not None else 0,
                                    int(s.normals.shape[0]) if s.normals is not None else 0, int(s.indices.shape[0]), s.material_id, s.light_id))
         materials = []
-        for m in c.mat_args:
+        models = opt.specular_models
+        for i, m in enumerate(c.mat_args):
             textures = [_native_texture(rb, cls, nch, t) for (cls, nch), t in zip(_material_textures(rb), m.textures)]
-            materials.append(rb.Material(*textures, m.compute_specular_lighting, m.two_sided, m.use_vertex_color))
+            # (the keyword only for a non-default lobe: a backend without one renders Blinn-Phong)
+            materials.append(rb.Material(*textures, m.compute_specular_lighting, m.two_sided, m.use_vertex_color,
+                                         **({} if models is None or not models[i] else {"specular_model": models[i]})))
         lights = [rb.AreaLight(l.shape_id, fp(l.intensity), l.two_sided, l.directly_visible) for l in c.light_args]
         envmap = None
         if c.env_args is not None:

@@ -132,11 +132,11 @@ static int render_pass(const rb_scene* scene_, const rb_options* opt, float* ima
     // The feature-free instantiation of the kernels (rb_kernels_lean.cu) serves the common configuration, and its diffuse-only refinement
     // (rb_kernels_diffuse.cu) the scenes of that configuration whose materials are all diffuse; `kern` holds the kernels of the chosen
     // instantiation, and every launch of one of them below goes through it.  The materials are read from the scene's host copies on every
-    // call: rb_scene_update may have changed their flags.
+    // call: rb_scene_update may have changed their flags.  Neither set has the GGX lobe (RB_GGX is false there).
     const bool lean_allowed = getenv("RB_NO_LEAN") == nullptr;       // (test hook: force the general kernels)
     const bool diffuse_allowed = getenv("RB_NO_DIFFUSE") == nullptr; // (test hook: force the lean kernels where the diffuse ones would run)
     const DevCamera& cam = scene->dev.cam;
-    const bool lean = lean_allowed && rp.only_radiance && !scene->dev.has_envmap && cam.type == RB_CAMERA_PERSPECTIVE && !cam.has_distortion &&
+    const bool lean = lean_allowed && !materials_use_ggx(scene->materials.data(), (int)scene->materials.size()) && rp.only_radiance && !scene->dev.has_envmap && cam.type == RB_CAMERA_PERSPECTIVE && !cam.has_distortion &&
                       cam.filter_type == RB_FILTER_BOX && cam.filter_width == 1.0f;
     const bool diffuse = lean && diffuse_allowed && materials_diffuse_only(scene->materials.data(), (int)scene->materials.size());
     const RenderKernels kern = diffuse ? rb_diffuse::render_kernels() : lean ? rb_lean::render_kernels() : render_kernels();

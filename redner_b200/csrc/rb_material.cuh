@@ -1,10 +1,11 @@
-// Textures and the BSDF (Lambert + Blinn-Phong microfacet lobe), sampling, pdf and the adjoint of the BSDF value.
+// Textures and the BSDF (Lambert + Blinn-Phong or GGX microfacet lobe), sampling, pdf and the adjoint of the BSDF value.
 //   get_texture_value / d_get_texture_value   src/texture.h:335-355 / :357-419 (trilinear mip: :53-140, :142-333)
 //   bsdf / d_bsdf                             src/material.h:353-449 / :451-692
 //   bsdf_sample                               src/material.h:702-811
 //   bsdf_pdf                                  src/material.h:1023-1093
 //   perturb_shading_frame (+adjoints)         src/material.h:273-351
 // d_bsdf_sample / d_bsdf_pdf are not on the path (commented out at src/path_contribution.cpp:410-412,:463-474).
+// The GGX lobe (rb_material::specular_model) has no reference counterpart; DESIGN.md section "GGX" defines it.
 #pragma once
 #include "rb_atomic.cuh"
 #include "rb_types.cuh"
@@ -193,6 +194,13 @@ inline bool materials_diffuse_only(const rb_material* m, int n) {
         if (m[i].compute_specular_lighting != 0 || m[i].use_vertex_color != 0 || m[i].normal_map.num_levels > 0) return false;
     return true;
 }
+// True when some material's specular lobe is GGX (RB_SPECULAR && !RB_VERTEX_COLOR && RB_GGX), i.e. when only the general and deterministic
+// kernels compute what the scene asks for.  Tests the fields themselves, so that it answers the same in every build.
+inline bool materials_use_ggx(const rb_material* m, int n) {
+    for (int i = 0; i < n; i++)
+        if (m[i].compute_specular_lighting != 0 && m[i].use_vertex_color == 0 && m[i].specular_model == RB_SPECULAR_GGX) return true;
+    return false;
+}
 RB_HD Real roughness_to_phong(Real r) { return rb_max(2 / r - 2, Real(0)); }
 RB_HD Real d_roughness_to_phong(Real r, Real d_e) { return (r > 0 && r <= 1) ? -2 * d_e / rb_sq(r) : Real(0); }
 
@@ -250,6 +258,63 @@ RB_HD Real smith_g1(V3 v, V3 n, Real roughness) {
     return (Real(3.535) * a + Real(2.181) * a2) / (1 + Real(2.276) * a + Real(2.577) * a2);
 }
 
+// ---------------------------------------------------------------- GGX lobe
+// RB_SPECULAR && !RB_VERTEX_COLOR && RB_GGX: the material's specular lobe is GGX (false in the lean and diffuse-only kernels).
+#define RB_GGX_LOBE(m) (RB_SPECULAR(m) && !RB_VERTEX_COLOR(m) && RB_GGX(m))
+// r is redner's roughness after its clamps; alpha^2 == r.  Every quantity is a function of the lobe's normal, wi and wo only, so that
+// the adjoint reaches the shading normal (and through it the normal map) and nothing else of the frame.
+// The lobe's normal: the (perturbed) shading normal, mirrored when a two-sided material is seen from below.
+RB_HD V3 ggx_normal(const rb_material& m, const BsdfCtx& c, V3 wi) { return m.two_sided && dot(wi, c.frame.n) < 0 ? -c.frame.n : c.frame.n; }
+// Smith Lambda (-1 + sqrt(1 + x)) / 2 with x = alpha^2 tan^2(theta_v), written x / (2 (1 + sqrt(1 + x))) and with sin^2 = |n x v|^2,
+// so that it keeps its digits at small alpha and near the normal.
+RB_HD Real ggx_lambda(V3 v, V3 n, Real r) {
+    Real c = dot(v, n);
+    Real x = r * length_sq(cross(n, v)) / (c * c);
+    return x / (2 * (1 + sqrt(1 + x)));
+}
+// NDF alpha^2 / (pi ((n.h)^2 (alpha^2 - 1) + 1)^2) for a unit h, written alpha^2 / (pi (alpha^2 (n.h)^2 + |n x h|^2)^2) (no cancellation).
+RB_HD Real ggx_ndf(V3 h, V3 n, Real r) {
+    Real hz = dot(h, n);
+    Real q = r * hz * hz + length_sq(cross(n, h));
+    return r / (RB_PI * q * q);
+}
+// The specular term of bsdf_eval: F(h.wo) D(h) G2(wi, wo) / (4 |n.wi|), height-correlated G2 = 1 / (1 + Lambda(wi) + Lambda(wo)).
+RB_HD V3 ggx_eval(const rb_material& m, const BsdfCtx& c, V3 ks, Real r, V3 wi, V3 wo) {
+    V3 n = ggx_normal(m, c, wi);
+    V3 h = normalize(wi + wo);
+    Real cwi = dot(n, wi);
+    if (!(cwi > 0 && dot(n, h) > 0)) return zero3();
+    Real G = 1 / (1 + ggx_lambda(wi, n, r) + ggx_lambda(wo, n, r));
+    V3 F = ks + (mk3(1, 1, 1) - ks) * pow(rb_max(1 - fabs(dot(h, wo)), Real(0)), Real(5));
+    return F * (ggx_ndf(h, n, r) * G / (4 * cwi));
+}
+// Density of ggx_sample over wo: the visible-normal density G1(wi) D(h) max(0, wi.h) / (n.wi) times the reflection Jacobian 1 / (4 wo.h).
+RB_HD Real ggx_pdf(const rb_material& m, const BsdfCtx& c, Real r, V3 wi, V3 wo) {
+    V3 n = ggx_normal(m, c, wi);
+    V3 h = normalize(wi + wo);
+    Real cwi = dot(n, wi);
+    if (!(cwi > 0 && dot(n, h) > 0)) return 0;
+    return ggx_ndf(h, n, r) / ((1 + ggx_lambda(wi, n, r)) * 4 * cwi);
+}
+// A half vector drawn from the visible normals seen from wi (spherical caps, Dupuy & Benyoub 2023, in the configuration stretched to
+// alpha = 1), in the local coordinates of c.frame; zero when wi lies below the lobe's normal.
+RB_HD V3 ggx_sample_half(const rb_material& m, const BsdfCtx& c, Real r, V3 wi, V2 suv) {
+    V3 wl = to_local(c.frame, wi);
+    const Real s = m.two_sided && wl.z < 0 ? Real(-1) : Real(1);
+    wl.z *= s;
+    if (!(wl.z > 0)) return zero3();
+    Real alpha = sqrt(r);
+    V3 ws = normalize(mk3(alpha * wl.x, alpha * wl.y, wl.z));
+    Real phi = 2 * RB_PI * suv.x;
+    Real z = (1 - suv.y) * (1 + ws.z) - ws.z;
+    Real sin_t = sqrt(rb_max(1 - z * z, Real(0)));
+    V3 hs = mk3(sin_t * cos(phi) + ws.x, sin_t * sin(phi) + ws.y, z + ws.z);
+    if (!(hs.z > 0)) return zero3();
+    V3 hl = normalize(mk3(alpha * hs.x, alpha * hs.y, hs.z));
+    hl.z *= s;
+    return hl;
+}
+
 RB_HD V3 bsdf_eval(const rb_material& m, const SurfacePoint& p, const MatTex& tx, V3 wi, V3 wo, Real min_rough) {
     BsdfCtx c = bsdf_ctx(m, p);
     Real geom_wi = dot(c.geom_n, wi), geom_wo = dot(c.geom_n, wo);
@@ -261,7 +326,9 @@ RB_HD V3 bsdf_eval(const rb_material& m, const SurfacePoint& p, const MatTex& tx
     Real roughness = rb_max(tx.rough, min_rough);
     V3 diffuse = kd * (sh_wo / RB_PI);
     V3 spec = zero3();
-    if (RB_SPECULAR(m) && !RB_VERTEX_COLOR(m)) {
+    if (RB_GGX_LOBE(m)) {
+        spec = ggx_eval(m, c, ks, rb_max(roughness, Real(1e-6)), wi, wo);
+    } else if (RB_SPECULAR(m) && !RB_VERTEX_COLOR(m)) {
         V3 h = normalize(wi + wo);
         V3 hl = to_local(c.frame, h);
         if (m.two_sided && hl.z < 0) hl = -hl;
@@ -293,7 +360,9 @@ RB_HD Real bsdf_pdf(const rb_material& m, const SurfacePoint& p, const MatTex& t
     Real diffuse_pdf = 0;
     if (pd > 0) diffuse_pdf = pd * sh_wo / RB_PI;
     Real spec_pdf = 0;
-    if (ps > 0) {
+    if (ps > 0 && RB_GGX_LOBE(m)) {
+        spec_pdf = ps * ggx_pdf(m, c, rb_max(rb_max(tx.rough, min_rough), Real(1e-6)), wi, wo);
+    } else if (ps > 0) {
         V3 h = normalize(wi + wo);
         // the reference projects on the UNPERTURBED frame here (src/material.h:1078); reproduced
         V3 hl = to_local(p.shading_frame, h);
@@ -332,6 +401,25 @@ RB_HD V3 bsdf_sample_dir(const rb_material& m, const SurfacePoint& p, const MatT
         wo_diff.dir_dy = mk3(Real(0.03), Real(0.03), Real(0.03));
         V3 dir = to_world(c.frame, local);
         if (dot(c.geom_n, dir) * geom_wi < 0) dir = to_world(c.frame, -local);
+        return dir;
+    } else if (RB_GGX_LOBE(m)) {
+        Real roughness = rb_max(rb_max(tx.rough, min_rough), Real(1e-6));
+        next_min_rough = rb_max(roughness, min_rough);
+        V3 hl = ggx_sample_half(m, c, roughness, wi, suv);
+        if (hl.z == 0) return zero3();
+        V3 h = to_world(c.frame, hl);
+        V3 dir = 2 * dot(wi, h) * h - wi;
+        // below the geometric surface eval is zero; a flipped direction would not have the density ggx_pdf gives it
+        if (dot(c.geom_n, dir) * geom_wi < 0) return zero3();
+        // the ray differential of the Blinn-Phong branch (it only selects mip levels)
+        V3 dmdx = p.dn_dx * hl.z, dmdy = p.dn_dy * hl.z;
+        V3 wi_dx = -wi_diff.dir_dx, wi_dy = -wi_diff.dir_dy;
+        Real wdm_dx = dot(wi_dx, h) + dot(wi, dmdx);
+        Real wdm_dy = dot(wi_dy, h) + dot(wi, dmdy);
+        wo_diff.org_dx = wi_diff.org_dx;
+        wo_diff.org_dy = wi_diff.org_dy;
+        wo_diff.dir_dx = 2 * (dot(wi, h) * dmdx + wdm_dx * h) - wi_dx;
+        wo_diff.dir_dy = 2 * (dot(wi, h) * dmdy + wdm_dy * h) - wi_dy;
         return dir;
     } else {
         Real roughness = rb_max(rb_max(tx.rough, min_rough), Real(1e-6));
@@ -385,7 +473,67 @@ RB_D void d_bsdf_eval(const rb_material& m, const rb_material& d_m, const Surfac
     d_n += wo * d_sh_wo;
 
     Real roughness = rb_max(rb_max(tx.rough, min_rough), Real(1e-6));
-    if (RB_SPECULAR(m) && !RB_VERTEX_COLOR(m)) {
+    if (RB_GGX_LOBE(m)) {
+        // ggx_eval with x_v = r |n x v|^2 / (n.v)^2, Lambda_v = (sqrt(1 + x_v) - 1) / 2, D = r / (pi q^2), q = r (n'.h)^2 + |n x h|^2,
+        // n' = sg n the lobe's normal
+        const Real sg = m.two_sided && dot(wi, n) < 0 ? Real(-1) : Real(1);
+        const V3 ns = n * sg;
+        V3 h = normalize(wi + wo);
+        Real cwi = dot(ns, wi), hz = dot(ns, h);
+        if (cwi > 0 && hz > 0) {
+            const Real r = roughness;
+            V3 nxh = cross(n, h), nxi = cross(n, wi), nxo = cross(n, wo);
+            Real q = r * hz * hz + length_sq(nxh);
+            Real D = r / (RB_PI * q * q);
+            Real ci = dot(n, wi), co = dot(n, wo);
+            Real xi = r * length_sq(nxi) / (ci * ci), xo = r * length_sq(nxo) / (co * co);
+            Real sqi = sqrt(1 + xi), sqo = sqrt(1 + xo);
+            Real G = 1 / (1 + xi / (2 * (1 + sqi)) + xo / (2 * (1 + sqo)));
+            Real cos_d = dot(h, wo);
+            Real cos5 = pow(rb_max(1 - cos_d, Real(0)), Real(5));
+            V3 one = mk3(1, 1, 1);
+            V3 F = ks + (one - ks) * cos5;
+            Real k = D * G / (4 * cwi);
+            V3 d_F = d_out * k;
+            Real d_k = sum(d_out * F);
+            Real d_D = d_k * G / (4 * cwi), d_G = d_k * D / (4 * cwi);
+            Real d_cwi = -d_k * k / cwi;
+            d_wi += d_cwi * ns;
+            d_n += (d_cwi * sg) * wi;
+            V3 d_ks = d_F * (1 - cos5);
+            Real d_cos5 = sum(d_F * (one - ks));
+            Real d_cos_d = -5 * d_cos5 * pow(rb_max(1 - cos_d, Real(0)), Real(4));
+            V3 d_h = d_cos_d * wo;
+            d_wo += d_cos_d * h;
+            Real d_r = 0;
+            Real d_lambda = -d_G * G * G; // dLambda / dx = 1 / (4 sqrt(1 + x))
+            auto d_x = [&](V3 v, V3 nxv, Real cv, Real x, Real d_xv) -> V3 {
+                d_r += d_xv * length_sq(nxv) / (cv * cv);
+                Real d_cv = -2 * d_xv * x / cv;
+                V3 d_v = d_cv * n;
+                d_n += d_cv * v;
+                d_cross(n, v, nxv * (2 * d_xv * r / (cv * cv)), d_n, d_v);
+                return d_v;
+            };
+            d_wi += d_x(wi, nxi, ci, xi, d_lambda / (4 * sqi));
+            d_wo += d_x(wo, nxo, co, xo, d_lambda / (4 * sqo));
+            Real d_q = -2 * d_D * D / q;
+            d_r += d_D / (RB_PI * q * q) + d_q * hz * hz;
+            Real d_hz = d_q * 2 * r * hz;
+            d_h += d_hz * ns;
+            d_n += (d_hz * sg) * h;
+            d_cross(n, h, nxh * (2 * d_q), d_n, d_h);
+            V3 d_wiwo = d_normalize(wi + wo, d_h);
+            d_wi += d_wiwo;
+            d_wo += d_wiwo;
+            d_slot[1] = d_ks;
+            slot_on |= 2u;
+            if (roughness > min_rough) {
+                d_slot[2] = mk3(d_r, 0, 0);
+                slot_on |= 4u;
+            }
+        }
+    } else if (RB_SPECULAR(m) && !RB_VERTEX_COLOR(m)) {
         V3 h = normalize(wi + wo);
         V3 hl = to_local(c.frame, h);
         bool flipped = false;

@@ -40,12 +40,16 @@ typedef float Real;
 #define RB_CAM_DISTORT(cam) false
 #define RB_ONLY_RADIANCE(rp) true
 #define RB_PIXEL_BOX(cam) true
+#define RB_GGX(m) false
 #else
 #define RB_ENVMAP(sc) ((sc).has_envmap != 0)
 #define RB_CAM_GENERAL(cam) ((cam).type != RB_CAMERA_PERSPECTIVE || (cam).has_distortion != 0)
 #define RB_CAM_DISTORT(cam) ((cam).has_distortion != 0)
 #define RB_ONLY_RADIANCE(rp) ((rp).only_radiance != 0)
 #define RB_PIXEL_BOX(cam) ((cam).filter_type == RB_FILTER_BOX && (cam).filter_width == 1.0f)
+// The GGX specular lobe (rb_material::specular_model) lives in the general and deterministic kernels only; rb_render keeps scenes that
+// use it off the lean and diffuse-only sets.
+#define RB_GGX(m) ((m).specular_model == RB_SPECULAR_GGX)
 #endif
 // Material features.  rb_kernels_diffuse.cu compiles the lean kernels once more with RB_DIFFUSE defined as well: no material
 // computes specular lighting, uses vertex colours or has a normal map -- the diffuse-only scenes of shape and pose optimisation.

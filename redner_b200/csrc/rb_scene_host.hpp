@@ -55,9 +55,12 @@ inline void host_setup_pixel_filter(const rb_pixel_filter& f, DevCamera& dc) {
     dc.filter_type = g.type;
     dc.filter_width = g.width;
 }
-// Index and pixel-filter checks of the descriptor; returns the error message, or null.
+// Index, pixel-filter and specular-model checks of the descriptor; returns the error message, or null.
 inline const char* host_check_scene_desc(const rb_scene_desc& desc) {
     if (const char* err = host_check_pixel_filter(desc)) return err;
+    for (int m = 0; m < desc.num_materials; m++)
+        if (desc.materials[m].specular_model != RB_SPECULAR_BLINN_PHONG && desc.materials[m].specular_model != RB_SPECULAR_GGX)
+            return "rb_scene_create: material specular_model must be RB_SPECULAR_BLINN_PHONG (0) or RB_SPECULAR_GGX (1)";
     for (int l = 0; l < desc.num_lights; l++)
         if (desc.lights[l].shape_id < 0 || desc.lights[l].shape_id >= desc.num_shapes) return "rb_scene_create: area light refers to an invalid shape";
     for (int s = 0; s < desc.num_shapes; s++) {

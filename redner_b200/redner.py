@@ -185,7 +185,8 @@ class TextureN(_Texture):
 
 class Material:  # src/redner.cpp:133-151, src/material.h:12-91
     def __init__(self, diffuse_reflectance, specular_reflectance, roughness, generic_texture, normal_map, compute_specular_lighting,
-                 two_sided, use_vertex_color):
+                 two_sided, use_vertex_color, specular_model=0):
+        """`specular_model` (redner_b200 extension): rb_specular_model, 0 for the reference's Blinn-Phong lobe, 1 for GGX."""
         m = L.rb_material()
         m.diffuse_reflectance = diffuse_reflectance._c
         m.specular_reflectance = specular_reflectance._c
@@ -195,6 +196,7 @@ class Material:  # src/redner.cpp:133-151, src/material.h:12-91
         m.compute_specular_lighting = int(bool(compute_specular_lighting))
         m.two_sided = int(bool(two_sided))
         m.use_vertex_color = int(bool(use_vertex_color))
+        m.specular_model = int(specular_model)
         self._c = m
 
     def _levels(self, t):

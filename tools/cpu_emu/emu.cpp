@@ -396,6 +396,13 @@ static int emu_render(const rb_scene* scene, const rb_options* opt, float* image
         return 1;
     }
 #endif
+#ifdef RB_LEAN
+    // nor does the library run its lean kernels for a GGX lobe
+    if (materials_use_ggx(scene->materials.data(), (int)scene->materials.size())) {
+        g_err = "rb_render: this build has no GGX specular lobe (specular_model)";
+        return 1;
+    }
+#endif
     const DevScene& sc = scene->dev;
     if (image && !rp.only_radiance) {
         for (int j = 0; j < ka.owned_rows; j++)
