@@ -361,6 +361,17 @@ int rb_exact_sum_test(const float* values, const int* slots, int n, int num_slot
 int rb_texture_test(const rb_texture* tex, const rb_texture* d_tex, const float* queries, int n, const float* d_values, float* values,
                     float* d_queries, void* stream);
 
+/* Test hook: n environment-map lookups and m samples, one per thread, through the functions the render kernels call (rb_envmap.cuh).
+ * `env` is turned into the scene's map exactly as rb_scene_create does.  queries: [n, 9] floats { dir, dir_dx, dir_dy } per lookup;
+ * values receives [n, 3] (envmap_eval) and pdfs, unless NULL, [n] (envmap_pdf of dir).  With d_out ([n, 3]) the adjoint
+ * (d_envmap_eval) scatters into d_values -- the map's levels, sizes and channels, zeroed by the caller, uv_scale may be NULL -- and, unless
+ * NULL, into d_w2e (16 floats, row-major 4x4); d_queries (may be NULL) receives { d_dir, d_dir_dx, d_dir_dy } per lookup.  samples: [m, 2]
+ * doubles (sx, sy) for envmap_sample; sample_dirs receives [m, 3].  Every buffer is memory of the current device; negative counts, a map
+ * without 3 channels or positive level sizes, and a gradient pyramid of another shape are refused, as is the double-precision build.
+ * Runs on `stream` (a cudaStream_t, NULL == legacy default stream) and synchronises it. */
+int rb_envmap_test(const rb_envmap* env, const rb_texture* d_values, float* d_w2e, const float* queries, int n, const float* d_out, float* values,
+                   float* pdfs, float* d_queries, const double* samples, int m, float* sample_dirs, void* stream);
+
 const char* rb_last_error(void);
 const char* rb_version(void);
 

@@ -510,6 +510,50 @@ def texture_test(tex, queries, d_values=None, d_tex=None):
     return values, d_queries
 
 
+def envmap_test(envmap, queries, d_out=None, d_values=None, d_w2e=None, samples=None, with_pdf=True):
+    """Environment-map lookups, adjoints, samples and pdfs through the functions the render kernels call (rb_envmap_test): test hook.
+    `envmap` is an EnvironmentMap, `d_values` a Texture3 gradient pyramid of the map's shape (zeroed by the caller; its uv_scale may be
+    NULL) and `d_w2e` a float32 tensor of at least 16 elements or None.  `queries` is an [N, 9] float32 tensor (dir, dir_dx, dir_dy) on
+    the map's device, which is made current; `samples` an [M, 2] float64 tensor (sx, sy) or None.  Returns ([N, 3] values, [N] pdfs or
+    None, [N, 9] d(queries) or None, [M, 3] sampled directions or None).  With `d_out` ([N, 3]) the adjoint scatters into `d_values`
+    and `d_w2e`."""
+    import torch
+    lib = L.load()
+    queries = queries.to(torch.float32).contiguous()
+    if queries.dim() != 2 or queries.shape[1] != 9:
+        raise ValueError("redner.envmap_test: queries must have shape [N, 9]")
+    n, dev = queries.shape[0], queries.device
+    values = torch.empty((n, 3), dtype=torch.float32, device=dev)
+    pdfs = torch.empty(n, dtype=torch.float32, device=dev) if with_pdf else None
+    d_queries = None
+    if d_out is not None:
+        d_out = d_out.to(torch.float32).contiguous()
+        if tuple(d_out.shape) != (n, 3):
+            raise ValueError("redner.envmap_test: d_out must have shape [N, 3]")
+        if d_values is None:
+            raise ValueError("redner.envmap_test: d_out needs d_values")
+        if d_w2e is not None and (d_w2e.dtype != torch.float32 or not d_w2e.is_contiguous() or d_w2e.numel() < 16):
+            raise ValueError("redner.envmap_test: d_w2e must be a contiguous float32 tensor of at least 16 elements")
+        d_queries = torch.empty((n, 9), dtype=torch.float32, device=dev)
+    m, sample_dirs = 0, None
+    if samples is not None:
+        samples = samples.to(device=dev, dtype=torch.float64).contiguous()
+        if samples.dim() != 2 or samples.shape[1] != 2:
+            raise ValueError("redner.envmap_test: samples must have shape [M, 2]")
+        m = samples.shape[0]
+        sample_dirs = torch.empty((m, 3), dtype=torch.float32, device=dev)
+    stream = 0
+    if queries.is_cuda:
+        torch.cuda.set_device(dev)
+        stream = torch.cuda.current_stream(dev).cuda_stream
+    ptr = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None  # noqa: E731
+    rc = lib.rb_envmap_test(C.byref(envmap._c), C.byref(d_values._c) if d_values is not None else None, ptr(d_w2e), ptr(queries), n, ptr(d_out),
+                            ptr(values), ptr(pdfs), ptr(d_queries), ptr(samples), m, ptr(sample_dirs), C.c_void_p(stream or 0))
+    if rc != 0:
+        raise RuntimeError("redner.envmap_test: " + L.last_error(lib))
+    return values, pdfs, d_queries, sample_dirs
+
+
 class DScene:  # src/redner.cpp:75-82
     def __init__(self, camera, shapes, materials, area_lights, envmap, use_gpu, gpu_index):
         d = L.rb_dscene_desc()

@@ -310,6 +310,64 @@ extern "C" int rb_texture_test(const rb_texture* tex, const rb_texture* d_tex, c
     }
     return 0;
 }
+// Environment-map lookups, adjoints, samples and pdfs through the same functions as the library's hook, one query after another (host
+// pointers; the scatter is the emulator's single-lane plain add).  The argument checks that do not involve device memory are the library's.
+extern "C" int rb_envmap_test(const rb_envmap* env, const rb_texture* d_values, float* d_w2e, const float* queries, int n, const float* d_out, float* values,
+                              float* pdfs, float* d_queries, const double* samples, int m, float* sample_dirs, void*) {
+    const char* err = nullptr;
+    if (n < 0 || m < 0) err = "negative number of queries or samples";
+    else if (env == nullptr) err = "null environment map";
+    else if (d_out != nullptr && d_values == nullptr) err = "d_out needs a gradient pyramid";
+    else if (env->values.channels != 3) err = "the map must have 3 channels";
+    else if (env->values.num_levels < 1 || env->values.num_levels > RB_MAX_MIP_LEVELS) err = "num_levels must be in [1, RB_MAX_MIP_LEVELS]";
+    else if (d_out != nullptr && (d_values->channels != 3 || d_values->num_levels != env->values.num_levels))
+        err = "the gradient pyramid must have the map's levels and channels";
+    for (int l = 0; err == nullptr && l < env->values.num_levels; l++) {
+        if (env->values.width[l] < 1 || env->values.height[l] < 1) err = "every level of the map needs a positive width and height";
+        else if (d_out != nullptr && (d_values->width[l] != env->values.width[l] || d_values->height[l] != env->values.height[l]))
+            err = "the gradient pyramid must have the map's level sizes";
+    }
+    if (err != nullptr) {
+        g_err = std::string("rb_envmap_test: ") + err;
+        return 1;
+    }
+    DevScene ds{};
+    host_setup_envmap(env, ds);
+    const DevEnvmap& e = ds.env;
+    for (int i = 0; i < n; i++) {
+        const float* q = queries + 9 * (size_t)i;
+        const V3 dir = mk3(q[0], q[1], q[2]);
+        RayDiff rd = zero_raydiff();
+        rd.dir_dx = mk3(q[3], q[4], q[5]);
+        rd.dir_dy = mk3(q[6], q[7], q[8]);
+        const V3 v = envmap_eval(e, dir, rd);
+        values[3 * (size_t)i] = v.x;
+        values[3 * (size_t)i + 1] = v.y;
+        values[3 * (size_t)i + 2] = v.z;
+        if (pdfs != nullptr) pdfs[i] = envmap_pdf(e, dir);
+        if (d_out == nullptr) continue;
+        const float* g = d_out + 3 * (size_t)i;
+        V3 d_dir = zero3();
+        RayDiff d_rd = zero_raydiff();
+        d_envmap_eval(e, dir, rd, mk3(g[0], g[1], g[2]), *d_values, d_w2e, d_dir, d_rd);
+        if (d_queries != nullptr) {
+            float* dq = d_queries + 9 * (size_t)i;
+            const V3 o[3] = {d_dir, d_rd.dir_dx, d_rd.dir_dy};
+            for (int k = 0; k < 3; k++) {
+                dq[3 * k] = o[k].x;
+                dq[3 * k + 1] = o[k].y;
+                dq[3 * k + 2] = o[k].z;
+            }
+        }
+    }
+    for (int i = 0; i < m; i++) {
+        const V3 d = envmap_sample(e, samples[2 * (size_t)i], samples[2 * (size_t)i + 1]);
+        sample_dirs[3 * (size_t)i] = d.x;
+        sample_dirs[3 * (size_t)i + 1] = d.y;
+        sample_dirs[3 * (size_t)i + 2] = d.z;
+    }
+    return 0;
+}
 extern "C" int rb_scene_edge_list(const rb_scene* sc, int* num_edges, int* edges_out, size_t edges_bytes) {
     if (num_edges) *num_edges = sc->dev.num_edges;
     if (edges_out && edges_bytes > 0) memcpy(edges_out, sc->et.edges.data(), std::min(edges_bytes, sizeof(Edge) * (size_t)sc->dev.num_edges));
