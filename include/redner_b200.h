@@ -274,7 +274,8 @@ int rb_scene_last_stats(const rb_scene* scene, int* num_kernel_launches, float* 
  * { k_forward, backward bands (trace + boundary terms + sweep), k_primary_edge, k_finish_camera } (0 for kernels that
  * did not run), the number of path
  * vertices at which the last backward pass formed a radiance estimate and its number of primary hits (mean executed
- * bounces per sample = path_vertices / (W*H*spp), SURVEY.md section 8d). */
+ * bounces per sample = path_vertices / (W*H*spp), SURVEY.md section 8d).  Both count the samples the backward pass traced:
+ * it skips the samples of pixels whose d_rendered_image is exactly zero in every float. */
 int rb_scene_last_stage_stats(const rb_scene* scene, float* stage_ms4, double* path_vertices, double* primary_hits);
 /* Split of the backward bands of the last rb_render, summed over the bands:
  * { k_bwd_trace, scan + compaction + k_bwd_secondary, k_bwd_sweep } in milliseconds. */

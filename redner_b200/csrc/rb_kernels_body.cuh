@@ -216,13 +216,16 @@ RB_D SampleId band_sample(const RenderParams& rp, long long I) {
 // boundary stage will look at it at all (secondary edges are only sampled until the first rough bounce, src/edge.cpp:1396-1401)
 // and which strategy its boundary sample takes: the first number of its edge-sampler point < 0.5 -> GATHER, else HIERARCHY
 // (the reference's own per-sample coin, src/edge.cpp:1461-1472); one bit per depth in `vmask`.
+// A sample whose pixel's adjoint is exactly zero adds nothing: it is not traced (it still reaches the phase barriers) and gets
+// nrec = -1, which keeps it out of every work list, so the boundary stage and the sweep never see it.
 __global__ void __launch_bounds__(RB_BLOCK_TRACE, RB_MIN_BLOCKS_TRACE) k_bwd_trace(const __grid_constant__ DevScene sc, const __grid_constant__ KernelArgs ka) {
     const RenderParams& rp = ka.rp;
     RB_BLOCK_LOOP(t, ka.band_n) {
         bool act = t < ka.band_n;
         SampleId id = band_sample(rp, ka.band_i0 + (act ? t : 0));
         VertexRec* recs = ka.records + (size_t)(act ? t : 0) * ka.rec_per_sample;
-        int n = bwd_trace(sc, rp, id.pixel, id.px, id.py, id.s, recs, 1, act);
+        const bool traced = act && !(ka.zero_cull && pixel_adjoint_is_zero(ka, id.pixel));
+        int n = bwd_trace(sc, rp, id.pixel, id.px, id.py, id.s, recs, 1, traced); // (-1 when not traced)
         if (!act) continue;
         ka.nrec[t] = n;
         if (ka.dpos != nullptr) {
@@ -469,7 +472,7 @@ __global__ void __launch_bounds__(256) k_prim_keys(const __grid_constant__ DevSc
         long long i;
         int s;
         prim_sample_id(ka.rp, t0 + t, i, s);
-        keys[t] = primary_edge_key(sc, ka.rp, i, s, dim_base);
+        keys[t] = primary_edge_key(sc, ka, i, s, dim_base);
         vals[t] = (unsigned)t;
     }
 }

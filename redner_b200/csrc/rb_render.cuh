@@ -5,6 +5,8 @@
 //   primary_edge_sample    src/edge.cpp:385-625 + src/pathtracer.cpp:766-942 + src/edge.cpp:700-783
 //   finish_camera          d_look_at_matrix / d_project tail, src/transform.h:29-71, src/camera.h:811-829
 #pragma once
+#include <cstdlib>
+
 #include "rb_edge.cuh"
 #include "rb_path.cuh"
 #include "rb_secondary.cuh"
@@ -27,6 +29,7 @@ struct KernelArgs {
     RenderParams rp;
     int lanes_per_pixel; // L
     int owned_rows;      // rows of the viewport this device renders
+    int zero_cull;       // backward: skip the samples of pixels whose adjoint is exactly zero (pixel_adjoint_is_zero)
     float* image;        // forward
     const float* d_image;
     float* screen_grad;
@@ -118,10 +121,21 @@ inline const char* setup_kernel_args(const rb_options& opt, const rb_camera& cam
     while (L * 2 <= 32 && L * 2 <= rp.spp) L *= 2;
     ka.lanes_per_pixel = L;
     ka.owned_rows = count_owned_rows(rp.vp_h, part, num_parts, rows_per_stripe);
+    ka.zero_cull = getenv("RB_NO_ZERO_CULL") == nullptr; // (test hook: trace every sample whatever its pixel's adjoint)
     ka.image = image;
     ka.d_image = d_image;
     ka.screen_grad = screen_grad;
     return nullptr;
+}
+// True iff all rp.nd floats of d_image at viewport pixel `pixel` compare equal to zero (-0 included; NaN and inf are not zero).
+// Every term the backward pass computes for a sample of such a pixel is a product with one of these floats, and the samplers are
+// pure functions of (pixel, sample, depth): its samples add exact zeros, and leaving them out changes no other sample.  All nd
+// floats are tested, not only radiance's, so that G-buffer channels and the rad_dim offset (reads inside [0, nd)) are covered.
+RB_HD bool pixel_adjoint_is_zero(const KernelArgs& ka, int pixel) {
+    const float* p = ka.d_image + (size_t)ka.rp.nd * pixel;
+    for (int k = 0; k < ka.rp.nd; k++)
+        if (p[k] != 0.0f) return false;
+    return true;
 }
 // rb_render's refusals under a pixel filter other than the 1-pixel box; returns the error message, or null.
 inline const char* check_pixel_filter_options(const DevCamera& cam, const rb_options& opt, const float* screen_grad) {
@@ -551,6 +565,7 @@ RB_D void bwd_sweep(const DevScene& sc, const KernelArgs& ka, int pixel, int px,
 // The three stages back to back for ONE sample: used by the host-compiled debug emulator (tools/cpu_emu) only.
 RB_D int backward_sample(const DevScene& sc, const KernelArgs& ka, int pixel, int px, int py, int s, VertexRec* recs, CamAcc& cam_acc) {
     const RenderParams& rp = ka.rp;
+    if (ka.zero_cull && pixel_adjoint_is_zero(ka, pixel)) return -1; // (like k_bwd_trace: the sample is not traced)
     int nrec = bwd_trace(sc, rp, pixel, px, py, s, recs, 1);
     if (nrec < 0) return -1;
     V3 dpos[RB_MAX_BOUNDARY_BOUNCES]; // (setup_backward rejects deeper paths when the stage runs)
@@ -758,12 +773,50 @@ RB_D bool primary_edge_pick(const DevScene& sc, const RenderParams& rp, long lon
     }
     return primary_edge_pick_nonlinear(sc, v0, v1, pk);
 }
+// Viewport pixel whose d_image a primary-edge point reads under the 1-pixel box (clamped to [0, vp_w] x [0, vp_h], like the reference).
+RB_HD void edge_point_pixel(const DevCamera& cam, D2 ept, int& xi, int& yi) {
+    xi = rb_clampi(int(ept.x * cam.width - cam.vp_beg[0]), 0, cam.vp_end[0] - cam.vp_beg[0]);
+    yi = rb_clampi(int(ept.y * cam.height - cam.vp_beg[1]), 0, cam.vp_end[1] - cam.vp_beg[1]);
+}
+// Viewport pixels [cx0, cx1] x [cy0, cy1] whose filter support holds the screen point p (empty when cx1 < cx0 or cy1 < cy0), and
+// p's offsets (x, y) from the centre of viewport pixel (0, 0): pixel c is reached when |offset - c| < the filter's radius.
+struct FilterReach {
+    double x, y;
+    int cx0, cx1, cy0, cy1;
+};
+RB_HD FilterReach filter_reach(const DevCamera& cam, const RenderParams& rp, D2 p) {
+    FilterReach f;
+    const double r = filter_radius(cam);
+    f.x = p.x * cam.width - cam.vp_beg[0] - 0.5;
+    f.y = p.y * cam.height - cam.vp_beg[1] - 0.5;
+    f.cx0 = rb_clampi((int)floor(f.x - r) + 1, 0, rp.vp_w);
+    f.cx1 = rb_clampi((int)ceil(f.x + r) - 1, -1, rp.vp_w - 1);
+    f.cy0 = rb_clampi((int)floor(f.y - r) + 1, 0, rp.vp_h);
+    f.cy1 = rb_clampi((int)ceil(f.y + r) - 1, -1, rp.vp_h - 1);
+    return f;
+}
+// True iff every d_image float that primary_edge_sample reads for the edge point `ept` is zero: the sample then adds nothing.  The
+// 1-pixel box reads edge_point_pixel's pixel, every other filter the pixels of its reach (filter_splat).
+RB_D bool edge_point_adjoint_is_zero(const DevScene& sc, const KernelArgs& ka, D2 ept) {
+    if (RB_PIXEL_BOX(sc.cam)) {
+        int xi, yi;
+        edge_point_pixel(sc.cam, ept, xi, yi);
+        return pixel_adjoint_is_zero(ka, yi * ka.rp.vp_w + xi);
+    }
+    const FilterReach f = filter_reach(sc.cam, ka.rp, ept);
+    for (int cy = f.cy0; cy <= f.cy1; cy++)
+        for (int cx = f.cx0; cx <= f.cx1; cx++)
+            if (!pixel_adjoint_is_zero(ka, cy * ka.rp.vp_w + cx)) return false;
+    return true;
+}
 // Sort key of a primary-edge sample: (edge, position along the edge).  Samples that are neighbours under this key
-// shoot nearly the same camera rays and scatter into the same two vertices; ~0u = contributes nothing.
-RB_D unsigned primary_edge_key(const DevScene& sc, const RenderParams& rp, long long i, int s, int dim_base) {
+// shoot nearly the same camera rays and scatter into the same two vertices; ~0u = contributes nothing (no edge point, or one
+// whose pixels' adjoint is zero).
+RB_D unsigned primary_edge_key(const DevScene& sc, const KernelArgs& ka, long long i, int s, int dim_base) {
     Sampler smp;
     PrimEdgePick pk;
-    if (!primary_edge_pick(sc, rp, i, s, dim_base, smp, pk)) return 0xffffffffu;
+    if (!primary_edge_pick(sc, ka.rp, i, s, dim_base, smp, pk)) return 0xffffffffu;
+    if (ka.zero_cull && edge_point_adjoint_is_zero(sc, ka, pk.ept)) return 0xffffffffu;
     int ebits = 1;
     while ((1 << ebits) < sc.num_edges && ebits < 31) ebits++;
     int tbits = 31 - ebits; // (the top bit stays clear so that no key equals ~0u)
@@ -775,15 +828,11 @@ RB_D unsigned primary_edge_key(const DevScene& sc, const RenderParams& rp, long 
 RB_D void filter_splat(const DevCamera& cam, const RenderParams& rp, const float* d_image, D2 p, float* out) {
     const int nd = rp.nd < RB_MAX_ND ? rp.nd : RB_MAX_ND;
     for (int k = 0; k < nd; k++) out[k] = 0.f;
-    const double r = filter_radius(cam);
-    // offsets from the centre of viewport pixel (0, 0); pixel c is reached when |offset - c| < r
-    const double x = p.x * cam.width - cam.vp_beg[0] - 0.5, y = p.y * cam.height - cam.vp_beg[1] - 0.5;
-    const int cx0 = rb_clampi((int)floor(x - r) + 1, 0, rp.vp_w), cx1 = rb_clampi((int)ceil(x + r) - 1, -1, rp.vp_w - 1);
-    const int cy0 = rb_clampi((int)floor(y - r) + 1, 0, rp.vp_h), cy1 = rb_clampi((int)ceil(y + r) - 1, -1, rp.vp_h - 1);
-    for (int cy = cy0; cy <= cy1; cy++) {
-        const double wy = filter_density(cam, y - cy);
-        for (int cx = cx0; cx <= cx1; cx++) {
-            const float w = (float)(wy * filter_density(cam, x - cx));
+    const FilterReach f = filter_reach(cam, rp, p);
+    for (int cy = f.cy0; cy <= f.cy1; cy++) {
+        const double wy = filter_density(cam, f.y - cy);
+        for (int cx = f.cx0; cx <= f.cx1; cx++) {
+            const float w = (float)(wy * filter_density(cam, f.x - cx));
             const float* px = d_image + (size_t)rp.nd * ((size_t)cy * rp.vp_w + cx);
             for (int k = 0; k < nd; k++) out[k] += w * px[k];
         }
@@ -796,13 +845,14 @@ RB_D void primary_edge_sample(const DevScene& sc, const KernelArgs& ka, long lon
     Sampler smp;
     PrimEdgePick pk;
     if (!primary_edge_pick(sc, rp, i, s, dim_base, smp, pk)) return;
+    if (ka.zero_cull && edge_point_adjoint_is_zero(sc, ka, pk.ept)) return; // (before any ray: k_prim_keys drops these samples too)
     const double pmf = pk.pmf;
     const D2 q0 = pk.q0, q1 = pk.q1, ept = pk.ept;
     const Edge edge = sc.edges[pk.edge_id];
     V3 v0 = edge_v0(sc.shapes, edge), v1 = edge_v1(sc.shapes, edge);
     int vp_w = rp.vp_w;
-    int xi = rb_clampi(int(ept.x * sc.cam.width - sc.cam.vp_beg[0]), 0, sc.cam.vp_end[0] - sc.cam.vp_beg[0]);
-    int yi = rb_clampi(int(ept.y * sc.cam.height - sc.cam.vp_beg[1]), 0, sc.cam.vp_end[1] - sc.cam.vp_beg[1]);
+    int xi, yi;
+    edge_point_pixel(sc.cam, ept, xi, yi);
     const float* dpx_all = ka.d_image + (size_t)rp.nd * ((size_t)yi * vp_w + xi);
     // Under a pixel filter the edge point weighs into every viewport pixel whose support holds it.  The integrand is linear in the
     // d_image multipliers, so the rays and the scatter below run once, on their filter-weighted sum.
