@@ -56,6 +56,14 @@ typedef struct rb_camera {
     float clip_near;
     int camera_type; /* rb_camera_type */
     int viewport_beg[2], viewport_end[2]; /* (x, y) -- src/camera.h:82 */
+    /* Thin lens (no reference counterpart; DESIGN.md "thin-lens camera"), in world units.  lens_radius == 0 (the zero-initialised
+     * struct) is the pinhole, and focus_distance is then ignored.  With lens_radius > 0 each camera sample also picks a point L on the
+     * disc of that radius around the camera origin, in the plane z = 0 of camera space, uniformly, and the ray leaves L towards the
+     * point of the plane z = focus_distance that the pinhole ray of the same film position meets.  rb_scene_create, rb_scene_update and
+     * rb_scene_set_camera refuse, with a message naming the lens, a lens_radius that is negative or not finite, a focus_distance that is
+     * not finite or not > 0, and a lens on anything but a perspective camera without distortion and with the 1-pixel box pixel filter;
+     * rb_render refuses a lens together with a screen_gradient_image. */
+    float lens_radius, focus_distance;
 } rb_camera;
 
 /* Shape -- src/shape.h:9-63.  All pointers are device pointers; optional ones may be NULL. */
@@ -180,6 +188,7 @@ typedef struct rb_dcamera {
     float *cam_to_world, *world_to_cam; /* 16 floats each */
     float *intrinsic_mat_inv, *intrinsic_mat; /* 9 floats each */
     float* distortion;                /* 8 floats or NULL */
+    float* lens;                      /* 2 floats { d(lens_radius), d(focus_distance) }, or NULL; written only when the camera has a lens */
 } rb_dcamera;
 
 /* DEnvironmentMap -- src/envmap.h:53-61: gradient mip pyramid and the 16 floats of d(world_to_env) (device memory) */

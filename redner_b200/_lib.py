@@ -34,6 +34,7 @@ class rb_camera(C.Structure):
         ("has_distortion", C.c_int), ("distortion", C.c_float * 8),
         ("clip_near", C.c_float), ("camera_type", C.c_int),
         ("viewport_beg", C.c_int * 2), ("viewport_end", C.c_int * 2),
+        ("lens_radius", C.c_float), ("focus_distance", C.c_float),
     ]
 
 
@@ -112,6 +113,7 @@ class rb_dcamera(C.Structure):
     _fields_ = [
         ("position", C.c_void_p), ("look", C.c_void_p), ("up", C.c_void_p), ("cam_to_world", C.c_void_p), ("world_to_cam", C.c_void_p),
         ("intrinsic_mat_inv", C.c_void_p), ("intrinsic_mat", C.c_void_p), ("distortion", C.c_void_p),
+        ("lens", C.c_void_p),
     ]
 
 

@@ -51,10 +51,16 @@ def set_use_correlated_random_number(v: bool):
 
 class Camera:
     def __init__(self, position=None, look_at=None, up=None, fov=None, clip_near: float = 1e-4, resolution: Tuple[int, int] = (256, 256),
-                 viewport=None, cam_to_world=None, intrinsic_mat=None, distortion_params=None, camera_type=0):
+                 viewport=None, cam_to_world=None, intrinsic_mat=None, distortion_params=None, camera_type=0, lens_radius=None,
+                 focus_distance=None):
+        """`lens_radius`, `focus_distance` (no reference counterpart): a thin lens, float32 tensors of shape (1,) in world units that may
+        require grad; None is the pinhole.  Rays leave a uniform point of the disc of radius lens_radius around the camera origin and pass
+        through the point of the plane at depth focus_distance that the pinhole ray of the same film position meets (DESIGN.md
+        "thin-lens camera").  A lens needs a perspective camera without distortion parameters and the 1-pixel box pixel filter."""
         if position is None and look_at is None and up is None:
             assert cam_to_world is not None
-        for t, n in ((position, 3), (look_at, 3), (up, 3), (fov, 1)):
+        assert (lens_radius is None) == (focus_distance is None), "give both lens_radius and focus_distance, or neither"
+        for t, n in ((position, 3), (look_at, 3), (up, 3), (fov, 1), (lens_radius, 1), (focus_distance, 1)):
             if t is not None:
                 assert t.dtype == torch.float32 and tuple(t.shape) == (n,)
         assert isinstance(clip_near, float)
@@ -76,6 +82,7 @@ class Camera:
         self.resolution = resolution  # (height, width)
         self.viewport = viewport      # (y0, x0, y1, x1) or None
         self.camera_type = camera_type
+        self.lens_radius, self.focus_distance = lens_radius, focus_distance
 
 
 class Texture:
@@ -222,7 +229,7 @@ _MaterialArgs = namedtuple("_MaterialArgs", "textures compute_specular_lighting 
 _LightArgs = namedtuple("_LightArgs", "shape_id intensity two_sided directly_visible")
 _EnvmapArgs = namedtuple("_EnvmapArgs", "values env_to_world world_to_env sample_cdf_ys sample_cdf_xs pdf_norm directly_visible")
 _OptionArgs = namedtuple("_OptionArgs", "num_samples max_bounces channels sampler_type use_primary_edge_sampling use_secondary_edge_sampling "
-                                        "sample_pixel_center pixel_filter device backend specular_models")
+                                        "sample_pixel_center pixel_filter device backend specular_models lens_radius focus_distance")
 
 
 def _ptr(backend, t, kind="float"):
@@ -322,7 +329,8 @@ class RenderFunction(torch.autograd.Function):
         if max_bounces == 0:
             use_secondary_edge_sampling = False
         vis = False  # does any parameter need discontinuity (edge) sampling? (render_pytorch.py:144-160)
-        for t in (cam.position, cam.look_at, cam.up, cam.cam_to_world, cam.world_to_cam, cam.intrinsic_mat, cam.intrinsic_mat_inv, cam.distortion_params):
+        lens = (getattr(cam, "lens_radius", None), getattr(cam, "focus_distance", None))
+        for t in (cam.position, cam.look_at, cam.up, cam.cam_to_world, cam.world_to_cam, cam.intrinsic_mat, cam.intrinsic_mat_inv, cam.distortion_params) + lens:
             if t is not None:
                 assert torch.isfinite(t).all()
                 vis = vis or t.requires_grad
@@ -367,6 +375,8 @@ class RenderFunction(torch.autograd.Function):
         # the materials' rb_specular_model values, None when every one is the default (the last entry, so that no other one moves)
         models = tuple(Material.SPECULAR_MODELS.index(getattr(m, "specular_model", "blinn_phong")) for m in scene.materials)
         args.append(models if any(models) else None)
+        # the thin lens: lens_radius and focus_distance, None for a pinhole (the last group, so that no other entry moves)
+        args += [t.cpu().contiguous() if t is not None else None for t in lens]
         return args
 
     @staticmethod
@@ -432,7 +442,9 @@ class RenderFunction(torch.autograd.Function):
         camera = rb.Camera(cam.resolution[1], cam.resolution[0], fp(cam.position if look_at else None), fp(cam.look_at if look_at else None),
                            fp(cam.up if look_at else None), fp(cam.cam_to_world), fp(cam.world_to_cam), fp(cam.intrinsic_mat_inv),
                            fp(cam.intrinsic_mat), fp(cam.distortion_params), cam.clip_near, rb.CameraType(int(cam.camera_type)),
-                           rb.Vector2i(vp[1], vp[0]), rb.Vector2i(vp[3], vp[2]))
+                           rb.Vector2i(vp[1], vp[0]), rb.Vector2i(vp[3], vp[2]),
+                           # (the keywords only with a lens: a backend without one renders the pinhole)
+                           **({} if opt.lens_radius is None else {"lens_radius": float(opt.lens_radius.detach()), "focus_distance": float(opt.focus_distance.detach())}))
         shapes = []
         for s in c.shape_args:
             assert s.vertices.is_contiguous() and s.indices.is_contiguous()
@@ -484,7 +496,8 @@ class RenderFunction(torch.autograd.Function):
         """Zeroed gradient buffers for every differentiable input of `c` (the unpacked call, or read_args' result alone), and the DScene
         that points at them (`.d_scene`).  `zeros(*shape)` allocates one buffer (default: torch.zeros on the render device).
 
-        The buffers, in the order they are allocated: `camera` (the eight of rb.DCamera, None where there is none), `shapes` ((vertices,
+        The buffers, in the order they are allocated: `camera` (the eight of rb.DCamera, None where there is none), `lens` (None for a
+        pinhole, else the two floats d(lens_radius), d(focus_distance) in one buffer, whose halves are the grads of the two entries), `shapes` ((vertices,
         uvs, normals, colors) per shape), `materials` (per material its five textures, each None or (mips, uv_scale)), `intensities` (per
         light) and `envmap` (None or (mips, uv_scale, world_to_env)).  `grads` maps the position in serialize_scene's list of each argument
         that has a buffer to that buffer."""
@@ -509,6 +522,11 @@ class RenderFunction(torch.autograd.Function):
                     None if look_at else buf(cp.cam_to_world, 4, 4), None if look_at else buf(cp.world_to_cam, 4, 4),
                     buf(cp.intrinsic_mat_inv, 3, 3), buf(cp.intrinsic_mat, 3, 3),
                     buf(cp.distortion_params, 8) if cam.distortion_params is not None else None)
+        opt, op = c.option_args, p.option_args
+        g.lens = None
+        if opt.lens_radius is not None:
+            g.lens = z(2)
+            g.grads[op.lens_radius], g.grads[op.focus_distance] = g.lens[0:1], g.lens[1:2]
         g.shapes = [(like(s.vertices, q.vertices), like(s.uvs, q.uvs), like(s.normals, q.normals), like(s.colors, q.colors))
                     for s, q in zip(c.shape_args, p.shape_args)]
         g.materials = [[texture(t, q) for t, q in zip(m.textures, mp.textures)] for m, mp in zip(c.mat_args, p.mat_args)]
@@ -520,7 +538,7 @@ class RenderFunction(torch.autograd.Function):
             d_envmap = rb.DEnvironmentMap(_native_texture(rb, rb.Texture3, 3, values, g.envmap[:2]), fp(g.envmap[2]))
         d_materials = [rb.DMaterial(*[_native_texture(rb, cls, nch, t, b) for (cls, nch), t, b in zip(_material_textures(rb), m.textures, bufs)])
                        for m, bufs in zip(c.mat_args, g.materials)]
-        g.d_scene = rb.DScene(rb.DCamera(*[fp(t) for t in g.camera]), [rb.DShape(*[fp(t) for t in b]) for b in g.shapes], d_materials,
+        g.d_scene = rb.DScene(rb.DCamera(*[fp(t) for t in g.camera], **({} if g.lens is None else {"lens": fp(g.lens)})), [rb.DShape(*[fp(t) for t in b]) for b in g.shapes], d_materials,
                               [rb.DAreaLight(fp(t)) for t in g.intensities], d_envmap, dev.type == "cuda", dev.index if dev.index is not None else -1)
         return g
 

@@ -195,10 +195,48 @@ RB_HD void cam_sample_primary_any(const DevCamera& cam, double sx_, double sy_, 
     }
 }
 
-// The common camera (pinhole, no lens model) has its own short path; everything else goes through the general one.
-RB_HD void cam_sample_primary(const DevCamera& cam, double sx, double sy, D3& org, D3& dir) {
+// ---- thin lens (rb_camera::lens_radius > 0, perspective cameras without distortion only; DESIGN.md "thin-lens camera") ----
+// A lens sample is the point `lu` of the unit disc; the lens point is L = lens_radius * (lu.x, lu.y, 0) in camera space.
+// Shirley-Chiu concentric map of [0, 1)^2 onto the unit disc: uniform, and continuous inside each of its four wedges.
+RB_HD D2 concentric_disc(double u1, double u2) {
+    const double a = 2.0 * u1 - 1.0, b = 2.0 * u2 - 1.0;
+    if (a == 0.0 && b == 0.0) return d2(0, 0);
+    const double quarter_pi = 0.78539816339744830962;
+    double r, phi;
+    if (a * a > b * b) {
+        r = a;
+        phi = quarter_pi * (b / a);
+    } else {
+        r = b;
+        phi = 2.0 * quarter_pi - quarter_pi * (a / b);
+    }
+    return d2(r * cos(phi), r * sin(phi));
+}
+// Ray of film position (sx, sy) through lens point lu: from L towards F = d f / d.z, the point of the focal plane z = f on the pinhole
+// ray d = intr_inv (px, py, 1).
+RB_HD void cam_sample_lens(const DevCamera& cam, double sx, double sy, D2 lu, D3& org, D3& dir) {
+    const double* C = cam.c2w;
+    const double* I = cam.intr_inv;
+    double aspect = double(cam.width) / double(cam.height);
+    double px = (sx - 0.5) * 2.0, py = (sy - 0.5) * (-2.0) / aspect, pz = 1.0;
+    D3 d = d3(I[0] * px + I[1] * py + I[2] * pz, I[3] * px + I[4] * py + I[5] * pz, I[6] * px + I[7] * py + I[8] * pz);
+    const double t = cam.focus_distance / d.z, lx = cam.lens_radius * lu.x, ly = cam.lens_radius * lu.y;
+    D3 n = d3_normalize(d3(d.x * t - lx, d.y * t - ly, d.z * t));
+    double iw = 1.0 / (C[12] * lx + C[13] * ly + C[15]);
+    org = d3((C[0] * lx + C[1] * ly + C[3]) * iw, (C[4] * lx + C[5] * ly + C[7]) * iw, (C[8] * lx + C[9] * ly + C[11]) * iw);
+    D3 w = d3(C[0] * n.x + C[1] * n.y + C[2] * n.z, C[4] * n.x + C[5] * n.y + C[6] * n.z, C[8] * n.x + C[9] * n.y + C[10] * n.z);
+    dir = d3_normalize(w);
+}
+
+// The common camera (pinhole, no lens model) has its own short path; everything else goes through the general one.  `lu` is the lens
+// sample of a camera with a lens, and unused otherwise.
+RB_HD void cam_sample_primary(const DevCamera& cam, double sx, double sy, D3& org, D3& dir, D2 lu = D2{0, 0}) {
     if (RB_CAM_GENERAL(cam)) {
         cam_sample_primary_any(cam, sx, sy, org, dir);
+        return;
+    }
+    if (RB_CAM_LENS(cam)) {
+        cam_sample_lens(cam, sx, sy, lu, org, dir);
         return;
     }
     const double* C = cam.c2w;
@@ -223,12 +261,13 @@ RB_HD Ray make_ray(D3 o, D3 d) {
 }
 
 // Primary ray + ray differential at normalised screen position (sx, sy).
-RB_HD void cam_primary_ray(const DevCamera& cam, double sx, double sy, Ray& ray, RayDiff& rd) {
+// With a lens all three rays leave the same lens point.
+RB_HD void cam_primary_ray(const DevCamera& cam, double sx, double sy, Ray& ray, RayDiff& rd, D2 lu = D2{0, 0}) {
     D3 o, d, ox, dx, oy, dy;
-    cam_sample_primary(cam, sx, sy, o, d);
+    cam_sample_primary(cam, sx, sy, o, d, lu);
     const double delta = 1e-3;
-    cam_sample_primary(cam, sx + delta, sy, ox, dx);
-    cam_sample_primary(cam, sx, sy + delta, oy, dy);
+    cam_sample_primary(cam, sx + delta, sy, ox, dx, lu);
+    cam_sample_primary(cam, sx, sy + delta, oy, dy, lu);
     double psx = 0.5 / cam.width, psy = 0.5 / cam.height;
     ray = make_ray(o, d);
     rd.org_dx = mk3((Real)(psx * (ox.x - o.x) / delta), (Real)(psx * (ox.y - o.y) / delta), (Real)(psx * (ox.z - o.z) / delta));
@@ -254,10 +293,12 @@ RB_HD M3 cam_m3(const double* a) {
 // <= 30 addresses (src/camera.h:244-259) -- its worst contention point.  Here every thread owns a strided
 // column in shared memory; the block reduces once at kernel end and issues one double atomic per scalar.
 // Layout (RB_CAM_ACC floats): [0..15] d_cam_to_world, [16..31] d_world_to_cam, [32..40] d_intr_inv, [41..49] d_intr,
-// [50..57] d_distortion.
+// [50..57] d_distortion, and with a lens [58] d_lens_radius, [59] d_focus_distance: cam_acc_count(cam) floats in all.
 // Deterministic mode (rb_kernels_det.cu) keeps one exact accumulator (rb_exact.cuh) per scalar for the whole block instead: each
 // (float) contribution goes there, the block flushes them into the global exact accumulators at kernel end.
 #define RB_CAM_ACC 58
+#define RB_CAM_ACC_LENS 60
+RB_HD int cam_acc_count(const DevCamera& cam) { return RB_CAM_LENS(cam) ? RB_CAM_ACC_LENS : RB_CAM_ACC; }
 struct CamAcc {
 #if defined(RB_DETERMINISTIC) && !defined(RB_CPU_EMU)
     long long* exact; // shared memory, [RB_CAM_ACC][RB_EXACT_WORDS]
@@ -297,7 +338,42 @@ struct CamAcc {
         for (int i = 0; i < 8; i++)
             if (d[i] != 0) add(50 + i, (Real)d[i]);
     }
+    RB_D void add_lens(Real d_radius, Real d_focus) {
+        if (d_radius != 0) add(58, d_radius);
+        if (d_focus != 0) add(59, d_focus);
+    }
 };
+
+// Adjoint of cam_sample_lens w.r.t. cam_to_world (the origin c2w (L, 1) included), intr_inv, lens_radius and focus_distance.
+RB_D void d_cam_sample_lens(const DevCamera& cam, Real sx, Real sy, D2 lu, const DRay& d_ray, CamAcc& acc) {
+    M4 C = cam_m4(cam.c2w);
+    M3 I = cam_m3(cam.intr_inv);
+    Real aspect = Real(cam.width) / Real(cam.height);
+    const Real r = (Real)cam.lens_radius, f = (Real)cam.focus_distance, ux = (Real)lu.x, uy = (Real)lu.y;
+    M4 d_C = zero_m4();
+    M3 d_I = zero_m3();
+    V3 L = mk3(r * ux, r * uy, 0);
+    V3 pt = mk3((sx - Real(0.5)) * 2, (sy - Real(0.5)) * (-2) / aspect, 1);
+    V3 d = mul(I, pt);
+    Real t = f / d.z;
+    V3 v = d * t - L;
+    V3 n_dir = normalize(v);
+    V3 world_dir = xfm_vector(C, n_dir);
+    V3 d_world_dir = d_normalize(world_dir, d_ray.dir);
+    V3 d_n_dir = zero3();
+    d_xfm_vector(C, n_dir, d_world_dir, d_C, d_n_dir);
+    V3 d_v = d_normalize(v, d_n_dir);
+    V3 d_d = d_v * t;
+    Real d_t = dot(d_v, d);
+    V3 d_L = -d_v;
+    Real d_f = d_t / d.z;
+    d_d.z -= d_t * t / d.z;
+    d_outer_acc(d_I, d_d, pt);
+    d_xfm_point(C, L, d_ray.org, d_C, d_L);
+    acc.add_intr_inv(d_I);
+    acc.add_c2w(d_C);
+    acc.add_lens(d_L.x * ux + d_L.y * uy, d_f);
+}
 
 // Adjoint of cam_sample_primary w.r.t. camera parameters (screen-position gradients are only needed for
 // distortion / screen_gradient_image; the latter is accumulated by the caller through d_screen).
@@ -393,9 +469,14 @@ RB_D void d_cam_sample_primary_any(const DevCamera& cam, Real sx_, Real sy_, con
     }
 }
 
-RB_D void d_cam_sample_primary(const DevCamera& cam, Real sx, Real sy, const DRay& d_ray, CamAcc& acc, V2* d_screen) {
+// (rb_render refuses a screen_gradient_image with a lens: d_screen is null there)
+RB_D void d_cam_sample_primary(const DevCamera& cam, Real sx, Real sy, const DRay& d_ray, CamAcc& acc, V2* d_screen, D2 lu = D2{0, 0}) {
     if (RB_CAM_GENERAL(cam)) {
         d_cam_sample_primary_any(cam, sx, sy, d_ray, acc, d_screen);
+        return;
+    }
+    if (RB_CAM_LENS(cam)) {
+        d_cam_sample_lens(cam, sx, sy, lu, d_ray, acc);
         return;
     }
     M4 C = cam_m4(cam.c2w);
@@ -582,6 +663,66 @@ RB_D void d_cam_project(const DevCamera& cam, V3 p0, V3 p1, Real dp0x, Real dp0y
     d_xfm_point(W, p1, d_b, d_W, d_p1);
     // d_cam_to_world = -W^T d_W W^T is applied once, at the end, on the reduced accumulator (it is linear in d_W).
     acc.add_w2c(d_W);
+}
+// Projection from the lens point L = (lx, ly, 0) with focal plane z = f: camera-space P lands where the pinhole screen map puts
+// Q = (lx / f + (P.x - lx) / P.z, ly / f + (P.y - ly) / P.z, 1), the point where the ray from L through P meets the focal plane, seen from
+// the origin.  For a fixed L it is a pinhole at L with a sheared frustum: lines stay lines on the film.
+RB_HD V3 lens_film_point(V3 P, Real lx, Real ly, Real f) { return mk3(lx / f + (P.x - lx) / P.z, ly / f + (P.y - ly) / P.z, 1); }
+RB_D void d_lens_film_point(const DevCamera& cam, V3 P, Real lx, Real ly, Real f, Real dx, Real dy, CamAcc& acc, V3& d_P, Real& d_lx, Real& d_ly, Real& d_f) {
+    V3 d_Q = zero3();
+    d_cam_to_screen(cam, lens_film_point(P, lx, ly, f), dx, dy, acc, d_Q);
+    d_P.x += d_Q.x / P.z;
+    d_P.y += d_Q.y / P.z;
+    d_P.z -= (d_Q.x * (P.x - lx) + d_Q.y * (P.y - ly)) / (P.z * P.z);
+    d_lx += d_Q.x * (1 / f - 1 / P.z);
+    d_ly += d_Q.y * (1 / f - 1 / P.z);
+    d_f -= (d_Q.x * lx + d_Q.y * ly) / (f * f);
+}
+// Adjoint of the projection of segment (p0, p1) from lens sample lu (cam_project_lens_d) w.r.t. the vertices, world_to_cam, intrinsic_mat,
+// lens_radius and focus_distance.  The near clip is the camera-space clip of cam_project, differentiated as written.
+RB_D void d_cam_project_lens(const DevCamera& cam, V3 p0, V3 p1, D2 lu, Real dp0x, Real dp0y, Real dp1x, Real dp1y, CamAcc& acc, V3& d_p0,
+                             V3& d_p1) {
+    M4 W = cam_m4(cam.w2c);
+    V3 a = xfm_point(W, p0), b = xfm_point(W, p1);
+    Real cn = cam.clip_near;
+    if (a.z < cn && b.z < cn) return;
+    V3 ca = a, cb = b;
+    if (a.z < cn) ca = b + ((cn - b.z) / (a.z - b.z)) * (a - b);
+    else if (b.z < cn) cb = a + ((cn - a.z) / (b.z - a.z)) * (b - a);
+    const Real r = (Real)cam.lens_radius, f = (Real)cam.focus_distance, ux = (Real)lu.x, uy = (Real)lu.y;
+    Real d_lx = 0, d_ly = 0, d_f = 0;
+    V3 d_ca = zero3(), d_cb = zero3();
+    d_lens_film_point(cam, ca, r * ux, r * uy, f, dp0x, dp0y, acc, d_ca, d_lx, d_ly, d_f);
+    d_lens_film_point(cam, cb, r * ux, r * uy, f, dp1x, dp1y, acc, d_cb, d_lx, d_ly, d_f);
+    V3 d_a = zero3(), d_b = zero3();
+    // clipped end c = q + t (p - q), t = (cn - q.z) / (p.z - q.z), p the end behind the plane
+    if (a.z < cn) {
+        V3 dir = a - b;
+        Real t = (cn - b.z) / dir.z, dt = dot(dir, d_ca);
+        V3 ddir = t * d_ca;
+        ddir.z -= dt * t / dir.z;
+        d_b += d_ca + ddir * Real(-1);
+        d_b.z -= dt / dir.z;
+        d_a += ddir;
+        d_b += d_cb;
+    } else if (b.z < cn) {
+        V3 dir = b - a;
+        Real t = (cn - a.z) / dir.z, dt = dot(dir, d_cb);
+        V3 ddir = t * d_cb;
+        ddir.z -= dt * t / dir.z;
+        d_a += d_cb + ddir * Real(-1);
+        d_a.z -= dt / dir.z;
+        d_b += ddir;
+        d_a += d_ca;
+    } else {
+        d_a += d_ca;
+        d_b += d_cb;
+    }
+    M4 d_W = zero_m4();
+    d_xfm_point(W, p0, d_a, d_W, d_p0);
+    d_xfm_point(W, p1, d_b, d_W, d_p1);
+    acc.add_w2c(d_W);
+    acc.add_lens(d_lx * ux + d_ly * uy, d_f);
 }
 RB_HD bool cam_in_screen(const DevCamera& cam, V2 pt) {
     int xi = int(pt.x * cam.width), yi = int(pt.y * cam.height);

@@ -116,8 +116,51 @@ RB_HD bool clip_line_filter(const DevCamera& cam, V2 v0, V2 v1, V2& a, V2& b) {
 }
 // Weight of an edge in the primary-edge distribution (src/edge.cpp:186-214): its screen-space length after clipping to the image (grown
 // by the pixel filter's reach) if it is a silhouette seen from the camera, else 0.
+// With a thin lens: positive for every edge that is a silhouette from some lens point and whose projection from that point meets the
+// image (only that makes the lens estimator unbiased).  On the film, the projection of camera-space P from lens point L is its projection
+// from the centre moved by the intrinsic scaling of L (1 / f - 1 / P.z), at most m(P.z) = r |1 / f - 1 / P.z| times that scaling in
+// screen units; 1 / z is monotone along a segment, so the near-clipped ends bound it.  The weight is the centre projection clipped to
+// the image grown by the larger bound, plus the two bounds.  The silhouette test keeps the edge unless the signed distance of the lens
+// point to each face plane, s(o) +- r |(n.ex, n.ey)| over the disc, stays strictly on one side and on the same side for both faces.
+RB_HD bool edge_is_lens_silhouette(const DevCamera& cam, const rb_shape* shapes, V3 org, const Edge& e) {
+    if (e.f0 == -1 || e.f1 == -1 || shapes[e.shape_id].normals == nullptr) return edge_is_silhouette(shapes, org, e);
+    V3 v0 = edge_v0(shapes, e), v1 = edge_v1(shapes, e);
+    V3 o0 = edge_opposite0(shapes, e), o1 = edge_opposite1(shapes, e);
+    V3 n0 = cross(v0 - o0, v1 - o0), n1 = cross(v1 - o1, v0 - o1);
+    Real l0 = length_sq(n0), l1 = length_sq(n1);
+    if (l0 < Real(1e-20) || l1 < Real(1e-20)) return false;
+    n0 = n0 / sqrt(l0);
+    n1 = n1 / sqrt(l1);
+    const V3 ex = mk3((Real)cam.c2w[0], (Real)cam.c2w[4], (Real)cam.c2w[8]), ey = mk3((Real)cam.c2w[1], (Real)cam.c2w[5], (Real)cam.c2w[9]);
+    const Real r = (Real)cam.lens_radius;
+    const Real s0 = dot(org - o0, n0), s1 = dot(org - o1, n1);
+    const Real h0 = r * sqrt(rb_sq(dot(n0, ex)) + rb_sq(dot(n0, ey))), h1 = r * sqrt(rb_sq(dot(n1, ex)) + rb_sq(dot(n1, ey)));
+    const bool front = s0 - h0 > 0 && s1 - h1 > 0, back = s0 + h0 < 0 && s1 + h1 < 0;
+    return !(front || back);
+}
+// Screen-space radius of the circle of confusion at camera depth z (the larger of its x and y extents).
+RB_HD Real lens_confusion_radius(const DevCamera& cam, Real z) {
+    const Real aspect = Real(cam.width) / Real(cam.height), k = (Real)fabs(cam.intr[8]);
+    const Real sx = Real(0.5) * ((Real)fabs(cam.intr[0]) + (Real)fabs(cam.intr[1])) / k, sy = Real(0.5) * aspect * ((Real)fabs(cam.intr[3]) + (Real)fabs(cam.intr[4])) / k;
+    return (Real)cam.lens_radius * (Real)fabs(Real(1) / (Real)cam.focus_distance - Real(1) / z) * (sx > sy ? sx : sy);
+}
+RB_HD double primary_edge_weight_lens(const DevCamera& cam, const rb_shape* shapes, const Edge& e, V3 org) {
+    V3 v0 = edge_v0(shapes, e), v1 = edge_v1(shapes, e);
+    M4 W = cam_m4(cam.w2c);
+    V3 a = xfm_point(W, v0), b = xfm_point(W, v1);
+    const Real cn = cam.clip_near;
+    if (a.z < cn && b.z < cn) return 0;
+    const Real za = a.z < cn ? cn : a.z, zb = b.z < cn ? cn : b.z;
+    const Real m0 = lens_confusion_radius(cam, za), m1 = lens_confusion_radius(cam, zb), g = m0 > m1 ? m0 : m1;
+    V2 p0, p1, c0, c1;
+    if (!cam_project(cam, v0, v1, p0, p1)) return 0;
+    if (!clip_line_unit(mk2((p0.x + g) / (1 + 2 * g), (p0.y + g) / (1 + 2 * g)), mk2((p1.x + g) / (1 + 2 * g), (p1.y + g) / (1 + 2 * g)), c0, c1)) return 0;
+    if (!edge_is_lens_silhouette(cam, shapes, org, e)) return 0;
+    return (double)(length(c1 - c0) * (1 + 2 * g) + m0 + m1);
+}
 RB_HD double primary_edge_weight(const DevCamera& cam, const rb_shape* shapes, const Edge& e) {
     double iw = 1.0 / cam.c2w[15];
+    if (RB_CAM_LENS(cam)) return primary_edge_weight_lens(cam, shapes, e, mk3((Real)(cam.c2w[3] * iw), (Real)(cam.c2w[7] * iw), (Real)(cam.c2w[11] * iw)));
     V3 org = mk3((Real)(cam.c2w[3] * iw), (Real)(cam.c2w[7] * iw), (Real)(cam.c2w[11] * iw));
     V3 v0 = edge_v0(shapes, e), v1 = edge_v1(shapes, e);
     V2 p0, p1, c0, c1;

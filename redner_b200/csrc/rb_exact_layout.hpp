@@ -1,5 +1,5 @@
 // The exact accumulators of one deterministic backward pass (rb_options::deterministic), shared by the CUDA driver (rb_kernels.cu)
-// and the host emulator (tools/cpu_emu): one accumulator per camera scalar (accumulators 0 .. RB_CAM_ACC - 1), then one per float of
+// and the host emulator (tools/cpu_emu): one accumulator per camera scalar (accumulators 0 .. cam_acc_count(cam) - 1), then one per float of
 // every gradient buffer the pass can write, and the gradient descriptors the kernels see in place of the caller's, whose buffer
 // pointers are virtual addresses of those accumulators (rb_exact.cuh).  A NULL pointer stays NULL.  Caller buffers that overlap share
 // accumulators: the memory ranges are merged before they are numbered, so every caller float has exactly one accumulator and the
@@ -61,8 +61,9 @@ inline void exact_layout(const rb_dscene_desc& d, const rb_shape* shapes, const 
     auto hash = [&](uint64_t v) {
         for (int b = 0; b < 8; b++) h = (h ^ ((v >> (8 * b)) & 0xffu)) * 1099511628211ull;
     };
-    hash(RB_CAM_ACC);
-    out.num_records = RB_CAM_ACC;
+    const int n_cam = cam_acc_count(sc.cam);
+    hash((uint64_t)n_cam);
+    out.num_records = n_cam;
     auto add = [&](const float* p, long long n) {
         const bool present = p != nullptr && n > 0;
         hash(present ? (uint64_t)n : 0);
@@ -104,7 +105,7 @@ inline void exact_layout(const rb_dscene_desc& d, const rb_shape* shapes, const 
     out.ranges.clear();
     out.rec_first.clear();
     out.overlaps = false;
-    out.num_acc = RB_CAM_ACC;
+    out.num_acc = n_cam;
     for (const Span& sp : spans) {
         if (!out.ranges.empty()) {
             ExactRange& r = out.ranges.back();

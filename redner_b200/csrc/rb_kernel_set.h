@@ -19,11 +19,11 @@ namespace rb_det {
 RenderKernels render_kernels();
 // Kernels of the exact accumulators (rb_exact.cuh), arguments as in rb_kernels_det.cu:
 //   normalise  (long long* acc, long long n)                                           carries of accumulators [0, n)
-//   finalise   (const long long* acc, long long n, const ExactRange* ranges, int num_ranges, double* cam_accum)
+//   finalise   (const long long* acc, long long n, const ExactRange* ranges, int num_ranges, double* cam_accum, int n_cam)
 //   sum_test   (const float* values, const int* slots, int n, long long j0, long long count)
 //   readout    (const long long* acc, int n, float* out_f32, double* out_f64)
-//   export_records  (const long long* acc, long long n, const ExactRange* ranges, const long long* rec_first, int num_ranges, long long* records)
-//   import_records  (long long* acc, long long n, const ExactRange* ranges, const long long* rec_first, int num_ranges, const long long* records)
+//   export_records  (const long long* acc, long long n, const ExactRange* ranges, const long long* rec_first, int num_ranges, long long* records, int n_cam)
+//   import_records  (long long* acc, long long n, const ExactRange* ranges, const long long* rec_first, int num_ranges, const long long* records, int n_cam)
 struct ExactKernels {
     const void *normalise, *finalise, *sum_test, *readout, *export_records, *import_records;
 };

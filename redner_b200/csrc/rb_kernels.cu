@@ -137,7 +137,7 @@ static int render_pass(const rb_scene* scene_, const rb_options* opt, float* ima
     const bool diffuse_allowed = getenv("RB_NO_DIFFUSE") == nullptr; // (test hook: force the lean kernels where the diffuse ones would run)
     const DevCamera& cam = scene->dev.cam;
     const bool lean = lean_allowed && !materials_use_ggx(scene->materials.data(), (int)scene->materials.size()) && rp.only_radiance && !scene->dev.has_envmap && cam.type == RB_CAMERA_PERSPECTIVE && !cam.has_distortion &&
-                      cam.filter_type == RB_FILTER_BOX && cam.filter_width == 1.0f;
+                      cam.filter_type == RB_FILTER_BOX && cam.filter_width == 1.0f && cam.lens_radius == 0;
     const bool diffuse = lean && diffuse_allowed && materials_diffuse_only(scene->materials.data(), (int)scene->materials.size());
     const RenderKernels kern = diffuse ? rb_diffuse::render_kernels() : lean ? rb_lean::render_kernels() : render_kernels();
     // Deterministic mode: the backward kernels of rb_kernels_det.cu (the forward kernels are deterministic as they are).  Records
@@ -202,7 +202,9 @@ static int render_pass(const rb_scene* scene_, const rb_options* opt, float* ima
             ka.ds.env_w2e = xl.env_w2e;
             ka.screen_grad = xl.screen_grad;
         }
-        const size_t cam_smem_sweep = det ? RB_SMEM_CAM_EXACT : RB_SMEM_CAM(RB_BLOCK_SWEEP), cam_smem_prim = det ? RB_SMEM_CAM_EXACT : RB_SMEM_CAM(RB_BLOCK_PRIM);
+        int n_cam = cam_acc_count(cam);
+        const size_t cam_smem_sweep = det ? RB_SMEM_CAM_EXACT(n_cam) : RB_SMEM_CAM(n_cam, RB_BLOCK_SWEEP),
+                     cam_smem_prim = det ? RB_SMEM_CAM_EXACT(n_cam) : RB_SMEM_CAM(n_cam, RB_BLOCK_PRIM);
         const long long exact_max_samples = exact_band_samples(rp.max_bounces);
         if (det && exact_max_samples < 1) {
             rb_set_error("rb_render: deterministic mode supports at most 2097150 bounces");
@@ -272,7 +274,7 @@ static int render_pass(const rb_scene* scene_, const rb_options* opt, float* ima
             exact_rec_first = (long long*)take(xo ? std::max<size_t>(xl.rec_first.size(), 1) * sizeof(long long) : 0);
             // Every pass starts with these three at zero.  They stay adjacent, carved one after the other, so that one memset clears them.
             const size_t zeroed_begin = off;
-            cam_accum = (double*)take(RB_CAM_ACC * sizeof(double));
+            cam_accum = (double*)take(RB_CAM_ACC_LENS * sizeof(double));
             counters = (BandCounters*)take((size_t)num_bands * sizeof(BandCounters));
             ka.edge_hist = (unsigned*)take(secondary ? n_edges * 4 : 0);
             zeroed_bytes = off - zeroed_begin;
@@ -407,12 +409,12 @@ static int render_pass(const rb_scene* scene_, const rb_options* opt, float* ima
         int num_ranges = (int)xl.ranges.size();
         if (xo) { // rb_render_exact: every accumulator, the camera's included, into the caller's records; no buffer of d_scene is written
             long long* records = xo->records;
-            void* exp_args[] = {&exact_acc, &n_acc, &exact_ranges, &exact_rec_first, &num_ranges, &records};
+            void* exp_args[] = {&exact_acc, &n_acc, &exact_ranges, &exact_rec_first, &num_ranges, &records, &n_cam};
             RB_CUDA_OK(cudaLaunchKernel(xk.export_records, grid_x, 256, exp_args, 0, stream));
             launches++;
         } else {
             if (det) { // round every accumulator once: into the caller's buffers, and the camera's into cam_accum
-                void* fin_args[] = {&exact_acc, &n_acc, &exact_ranges, &num_ranges, &cam_accum};
+                void* fin_args[] = {&exact_acc, &n_acc, &exact_ranges, &num_ranges, &cam_accum, &n_cam};
                 RB_CUDA_OK(cudaLaunchKernel(xk.finalise, grid_x, 256, fin_args, 0, stream));
                 launches++;
             }
@@ -527,7 +529,7 @@ extern "C" int rb_exact_round(const rb_scene* scene, const rb_options* opt, cons
     const size_t rec_bytes = align(std::max<size_t>(xl.rec_first.size(), 1) * sizeof(long long));
     DeviceScratch& dscratch = g_scratch[scene->device & 63];
     std::lock_guard<std::mutex> lock(dscratch.mutex);
-    char* scratch = scratch_ensure(dscratch, acc_bytes + range_bytes + rec_bytes + RB_CAM_ACC * sizeof(double));
+    char* scratch = scratch_ensure(dscratch, acc_bytes + range_bytes + rec_bytes + RB_CAM_ACC_LENS * sizeof(double));
     if (!scratch) {
         rb_set_error("rb_exact_round: out of device memory for the exact accumulators");
         return 1;
@@ -540,14 +542,15 @@ extern "C" int rb_exact_round(const rb_scene* scene, const rb_options* opt, cons
         RB_CUDA_OK(cudaMemcpyAsync(ranges, xl.ranges.data(), xl.ranges.size() * sizeof(ExactRange), cudaMemcpyHostToDevice, stream));
         RB_CUDA_OK(cudaMemcpyAsync(rec_first, xl.rec_first.data(), xl.rec_first.size() * sizeof(long long), cudaMemcpyHostToDevice, stream));
     }
-    RB_CUDA_OK(cudaMemsetAsync(cam_accum, 0, RB_CAM_ACC * sizeof(double), stream));
+    RB_CUDA_OK(cudaMemsetAsync(cam_accum, 0, RB_CAM_ACC_LENS * sizeof(double), stream));
     const rb_det::ExactKernels xk = rb_det::exact_kernels();
     long long n_acc = xl.num_acc;
     int num_ranges = (int)xl.ranges.size();
-    void* imp_args[] = {&acc, &n_acc, &ranges, &rec_first, &num_ranges, (void*)&records};
+    int n_cam = cam_acc_count(scene->dev.cam);
+    void* imp_args[] = {&acc, &n_acc, &ranges, &rec_first, &num_ranges, (void*)&records, &n_cam};
     RB_CUDA_OK(cudaLaunchKernel(xk.import_records, sms * 4, 256, imp_args, 0, stream));
     // from here on the end of a deterministic rb_render: round every accumulator once, then the camera
-    void* fin_args[] = {&acc, &n_acc, &ranges, &num_ranges, &cam_accum};
+    void* fin_args[] = {&acc, &n_acc, &ranges, &num_ranges, &cam_accum, &n_cam};
     RB_CUDA_OK(cudaLaunchKernel(xk.finalise, sms * 4, 256, fin_args, 0, stream));
     k_finish_camera<<<1, 32, 0, stream>>>(scene->dev.cam, cam_accum, d_scene->camera);
     RB_CUDA_OK(cudaStreamSynchronize(stream));

@@ -12,10 +12,10 @@ constexpr int RB_BLOCK_TRACE = 256, RB_MIN_BLOCKS_TRACE = 3; // k_bwd_trace
 constexpr int RB_BLOCK_SEC = 128, RB_MIN_BLOCKS_SEC = 6;     // k_bwd_sec_pick, k_bwd_sec_shade: 24 warps / SM at <= 80 registers
 constexpr int RB_BLOCK_SWEEP = 512, RB_MIN_BLOCKS_SWEEP = 1; // k_bwd_sweep
 constexpr int RB_BLOCK_PRIM = 128, RB_MIN_BLOCKS_PRIM = 5;   // k_primary_edge
-// dynamic shared memory: per-thread columns of the camera accumulators (k_bwd_sweep, k_primary_edge)
-#define RB_SMEM_CAM(block) ((size_t)RB_CAM_ACC * (block) * sizeof(float))
-// ... in the deterministic instantiation: the block's exact camera accumulators, [RB_CAM_ACC][RB_EXACT_WORDS]
-#define RB_SMEM_CAM_EXACT ((size_t)RB_CAM_ACC * RB_EXACT_WORDS * sizeof(long long))
+// dynamic shared memory: per-thread columns of the n_cam = cam_acc_count(cam) camera accumulators (k_bwd_sweep, k_primary_edge)
+#define RB_SMEM_CAM(n_cam, block) ((size_t)(n_cam) * (block) * sizeof(float))
+// ... in the deterministic instantiation: the block's exact camera accumulators, [n_cam][RB_EXACT_WORDS]
+#define RB_SMEM_CAM_EXACT(n_cam) ((size_t)(n_cam) * RB_EXACT_WORDS * sizeof(long long))
 #ifndef RB_BAND_BYTES
 #define RB_BAND_BYTES (1ULL << 30) // scratch budget of one backward band (records + lists)
 #endif
@@ -51,7 +51,7 @@ RB_D WorkItem warp_work(const RenderParams& rp, int L, int owned_rows, long long
 #define RB_TMA_SOBOL_DIMS 32
 RB_D unsigned rb_smem_addr(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
 RB_D const unsigned long long* stage_sobol_rows(const DevScene& sc, const RenderParams& rp, unsigned long long* smem_rows, unsigned long long* mbar) {
-    const int dims = (rp.sample_pixel_center ? 0 : 2) + 7 * rp.max_bounces;
+    const int dims = (int)main_draws_per_sample(sc, rp);
     if (rp.sampler_type != RB_SAMPLER_SOBOL || dims > RB_TMA_SOBOL_DIMS || dims == 0) return sc.sobol_matrices;
     const unsigned bytes = (unsigned)(dims * RB_SOBOL_BITS * sizeof(unsigned long long)); // 416 B per dimension: a multiple of 16
     const unsigned bar = rb_smem_addr(mbar), dst = rb_smem_addr(smem_rows);
@@ -161,11 +161,11 @@ __global__ void __launch_bounds__(RB_BLOCK, 2) k_forward_channels(const __grid_c
 
 #endif
 // ------------------------------------------------------------------------------------------------ backward (interior + first hit)
-RB_D void block_reduce_camera(float* cam_smem, double* cam_accum) {
-    // cam_smem: [RB_CAM_ACC][blockDim.x]; reduce each row and add to the global double accumulators
+RB_D void block_reduce_camera(float* cam_smem, double* cam_accum, int n_cam) {
+    // cam_smem: [n_cam][blockDim.x]; reduce each row and add to the global double accumulators
     __syncthreads();
     int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
-    for (int k = warp; k < RB_CAM_ACC; k += nw) {
+    for (int k = warp; k < n_cam; k += nw) {
         float s = 0.f;
         for (int i = lane; i < (int)blockDim.x; i += 32) s += cam_smem[k * blockDim.x + i];
         for (int off = 16; off > 0; off >>= 1) s += __shfl_xor_sync(0xffffffffu, s, off);
@@ -173,15 +173,15 @@ RB_D void block_reduce_camera(float* cam_smem, double* cam_accum) {
     }
 }
 #ifdef RB_DETERMINISTIC
-// Deterministic mode: the block's exact camera accumulators (shared memory, [RB_CAM_ACC][RB_EXACT_WORDS]) start at zero and end in
-// the global exact accumulators 0 .. RB_CAM_ACC - 1, normalised first so that a block adds less than 2^32 to each limb.
-RB_D void exact_camera_begin(long long* cam_exact) {
-    for (int i = threadIdx.x; i < RB_CAM_ACC * RB_EXACT_WORDS; i += blockDim.x) cam_exact[i] = 0;
+// Deterministic mode: the block's exact camera accumulators (shared memory, [n_cam][RB_EXACT_WORDS]) start at zero and end in
+// the global exact accumulators 0 .. n_cam - 1, normalised first so that a block adds less than 2^32 to each limb.
+RB_D void exact_camera_begin(long long* cam_exact, int n_cam) {
+    for (int i = threadIdx.x; i < n_cam * RB_EXACT_WORDS; i += blockDim.x) cam_exact[i] = 0;
     __syncthreads();
 }
-RB_D void exact_camera_flush(long long* cam_exact) {
+RB_D void exact_camera_flush(long long* cam_exact, int n_cam) {
     __syncthreads();
-    for (int k = threadIdx.x; k < RB_CAM_ACC; k += blockDim.x) {
+    for (int k = threadIdx.x; k < n_cam; k += blockDim.x) {
         long long a[RB_EXACT_WORDS];
         for (int i = 0; i < RB_EXACT_WORDS; i++) a[i] = cam_exact[k * RB_EXACT_WORDS + i];
         exact_normalise(a);
@@ -426,14 +426,15 @@ __global__ void __launch_bounds__(RB_BLOCK_SEC, RB_MIN_BLOCKS_SEC) k_bwd_sec_sha
 }
 // Stage 3: reverse sweep of every path, first-hit and camera adjoints.
 __global__ void __launch_bounds__(RB_BLOCK_SWEEP, RB_MIN_BLOCKS_SWEEP) k_bwd_sweep(const __grid_constant__ DevScene sc, const __grid_constant__ KernelArgs ka) {
+    const int n_cam = cam_acc_count(sc.cam);
 #ifdef RB_DETERMINISTIC
-    extern __shared__ long long cam_exact[]; // [RB_CAM_ACC][RB_EXACT_WORDS]
-    exact_camera_begin(cam_exact);
+    extern __shared__ long long cam_exact[]; // [n_cam][RB_EXACT_WORDS]
+    exact_camera_begin(cam_exact, n_cam);
     CamAcc cam_acc;
     cam_acc.exact = cam_exact;
 #else
-    extern __shared__ float cam_smem[]; // [RB_CAM_ACC][blockDim.x]
-    for (int k = 0; k < RB_CAM_ACC; k++) cam_smem[k * blockDim.x + threadIdx.x] = 0.f;
+    extern __shared__ float cam_smem[]; // [n_cam][blockDim.x]
+    for (int k = 0; k < n_cam; k++) cam_smem[k * blockDim.x + threadIdx.x] = 0.f;
     CamAcc cam_acc;
     cam_acc.base = cam_smem + threadIdx.x;
     cam_acc.stride = blockDim.x;
@@ -448,9 +449,9 @@ __global__ void __launch_bounds__(RB_BLOCK_SWEEP, RB_MIN_BLOCKS_SWEEP) k_bwd_swe
         bwd_sweep(sc, ka, id.pixel, id.px, id.py, id.s, ka.records + base, 1, act ? ka.nrec[ts] : 0, ka.dpos ? ka.dpos + base : nullptr, cam_acc, act);
     }
 #ifdef RB_DETERMINISTIC
-    exact_camera_flush(cam_exact);
+    exact_camera_flush(cam_exact, n_cam);
 #else
-    block_reduce_camera(cam_smem, ka.ds.cam_accum);
+    block_reduce_camera(cam_smem, ka.ds.cam_accum, n_cam);
 #endif
 }
 
@@ -478,14 +479,15 @@ __global__ void __launch_bounds__(256) k_prim_keys(const __grid_constant__ DevSc
 }
 __global__ void __launch_bounds__(RB_BLOCK_PRIM, RB_MIN_BLOCKS_PRIM) k_primary_edge(const __grid_constant__ DevScene sc, const __grid_constant__ KernelArgs ka, int dim_base,
                                                                                long long t0, int n, const unsigned* keys, const unsigned* vals) {
+    const int n_cam = cam_acc_count(sc.cam);
 #ifdef RB_DETERMINISTIC
-    extern __shared__ long long cam_exact[]; // [RB_CAM_ACC][RB_EXACT_WORDS]
-    exact_camera_begin(cam_exact);
+    extern __shared__ long long cam_exact[]; // [n_cam][RB_EXACT_WORDS]
+    exact_camera_begin(cam_exact, n_cam);
     CamAcc cam_acc;
     cam_acc.exact = cam_exact;
 #else
-    extern __shared__ float cam_smem[]; // [RB_CAM_ACC][blockDim.x]
-    for (int k = 0; k < RB_CAM_ACC; k++) cam_smem[k * blockDim.x + threadIdx.x] = 0.f;
+    extern __shared__ float cam_smem[]; // [n_cam][blockDim.x]
+    for (int k = 0; k < n_cam; k++) cam_smem[k * blockDim.x + threadIdx.x] = 0.f;
     CamAcc cam_acc;
     cam_acc.base = cam_smem + threadIdx.x;
     cam_acc.stride = blockDim.x;
@@ -500,9 +502,9 @@ __global__ void __launch_bounds__(RB_BLOCK_PRIM, RB_MIN_BLOCKS_PRIM) k_primary_e
         }
     }
 #ifdef RB_DETERMINISTIC
-    exact_camera_flush(cam_exact);
+    exact_camera_flush(cam_exact, n_cam);
 #else
-    block_reduce_camera(cam_smem, ka.ds.cam_accum);
+    block_reduce_camera(cam_smem, ka.ds.cam_accum, n_cam);
 #endif
 }
 

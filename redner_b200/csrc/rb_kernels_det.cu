@@ -36,20 +36,22 @@ __global__ void k_exact_normalise(long long* acc, long long n) {
 }
 // End of a deterministic backward pass: every accumulator that received something is rounded once (exact_finalise); the camera's
 // become the doubles k_finish_camera reads.
-__global__ void k_exact_finalise(const long long* acc, long long n, const ExactRange* ranges, int num_ranges, double* cam_accum) {
+__global__ void k_exact_finalise(const long long* acc, long long n, const ExactRange* ranges, int num_ranges, double* cam_accum, int n_cam) {
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
-        exact_finalise(acc, i, ranges, num_ranges, cam_accum, RB_CAM_ACC);
+        exact_finalise(acc, i, ranges, num_ranges, cam_accum, n_cam);
 }
 // rb_render_exact: every accumulator [0, n) is added into its record and the record left normalised (exact_export).  Accumulators
 // and records are disjoint one-to-one (the layout refuses overlapping buffers), so no two threads touch one record.
-__global__ void k_exact_export(const long long* acc, long long n, const ExactRange* ranges, const long long* rec_first, int num_ranges, long long* records) {
+__global__ void k_exact_export(const long long* acc, long long n, const ExactRange* ranges, const long long* rec_first, int num_ranges, long long* records,
+                               int n_cam) {
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
-        exact_export(acc + i * RB_EXACT_WORDS, records + exact_record_of(i, ranges, rec_first, num_ranges, RB_CAM_ACC) * RB_EXACT_RECORD_WORDS);
+        exact_export(acc + i * RB_EXACT_WORDS, records + exact_record_of(i, ranges, rec_first, num_ranges, n_cam) * RB_EXACT_RECORD_WORDS);
 }
 // rb_exact_round: accumulators [0, n) from their records (exact_import), ready for k_exact_finalise.
-__global__ void k_exact_import(long long* acc, long long n, const ExactRange* ranges, const long long* rec_first, int num_ranges, const long long* records) {
+__global__ void k_exact_import(long long* acc, long long n, const ExactRange* ranges, const long long* rec_first, int num_ranges, const long long* records,
+                               int n_cam) {
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
-        exact_import(records + exact_record_of(i, ranges, rec_first, num_ranges, RB_CAM_ACC) * RB_EXACT_RECORD_WORDS, acc + i * RB_EXACT_WORDS);
+        exact_import(records + exact_record_of(i, ranges, rec_first, num_ranges, n_cam) * RB_EXACT_RECORD_WORDS, acc + i * RB_EXACT_WORDS);
 }
 // Test hook rb_exact_sum_test: contribution j of [j0, j0 + count) adds values[j % n] to slot slots[j % n] through the scatter of the
 // render kernels (rb_red_add: the same warp aggregation and integer reductions), slot s being accumulator s.

@@ -41,6 +41,7 @@ typedef float Real;
 #define RB_ONLY_RADIANCE(rp) true
 #define RB_PIXEL_BOX(cam) true
 #define RB_GGX(m) false
+#define RB_CAM_LENS(cam) false
 #else
 #define RB_ENVMAP(sc) ((sc).has_envmap != 0)
 #define RB_CAM_GENERAL(cam) ((cam).type != RB_CAMERA_PERSPECTIVE || (cam).has_distortion != 0)
@@ -50,6 +51,8 @@ typedef float Real;
 // The GGX specular lobe (rb_material::specular_model) lives in the general and deterministic kernels only; rb_render keeps scenes that
 // use it off the lean and diffuse-only sets.
 #define RB_GGX(m) ((m).specular_model == RB_SPECULAR_GGX)
+// The thin lens (rb_camera::lens_radius) likewise: rb_render keeps lens cameras off the lean and diffuse-only sets.
+#define RB_CAM_LENS(cam) ((cam).lens_radius > 0)
 #endif
 // Material features.  rb_kernels_diffuse.cu compiles the lean kernels once more with RB_DIFFUSE defined as well: no material
 // computes specular lighting, uses vertex colours or has a normal map -- the diffuse-only scenes of shape and pose optimisation.

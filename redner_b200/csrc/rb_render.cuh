@@ -139,6 +139,7 @@ RB_HD bool pixel_adjoint_is_zero(const KernelArgs& ka, int pixel) {
 }
 // rb_render's refusals under a pixel filter other than the 1-pixel box; returns the error message, or null.
 inline const char* check_pixel_filter_options(const DevCamera& cam, const rb_options& opt, const float* screen_grad) {
+    if (cam.lens_radius > 0 && screen_grad != nullptr) return "rb_render: a screen_gradient_image needs a camera without a lens (lens_radius 0)";
     if (cam.filter_type == RB_FILTER_BOX && cam.filter_width == 1.0f) return nullptr;
     if (opt.sample_pixel_center) return "rb_render: sample_pixel_center needs the 1-pixel box pixel filter (the scene's filter places samples around the centre)";
     if (screen_grad != nullptr) return "rb_render: a screen_gradient_image needs the 1-pixel box pixel filter";
@@ -183,13 +184,14 @@ RB_HD void write_gbuffer_pixel(const RenderParams& rp, const float* acc, const i
     }
 }
 
-RB_HD unsigned long long main_draws_per_sample(const RenderParams& rp) {
-    return (unsigned long long)((rp.sample_pixel_center ? 0 : 2) + 7 * rp.max_bounces);
+// Main-sampler dimensions per sample: camera (2, or 0 with sample_pixel_center) | lens (2, with a lens only) | 7 per bounce.
+RB_HD unsigned long long main_draws_per_sample(const DevScene& sc, const RenderParams& rp) {
+    return (unsigned long long)((rp.sample_pixel_center ? 0 : 2) + (RB_CAM_LENS(sc.cam) ? 2 : 0) + 7 * rp.max_bounces);
 }
 // Edge-sampler dimension layout per sample, in the order of the reference's next_* calls on `edge_sampler`
 // (src/pathtracer.cpp:505, :630-641 inside the reverse depth loop, then :788, :871-882):
 //   for depth = mb-1 .. 0:  secondary edge (4) + 7 per remaining bounce of its two sub-paths
-//   primary edge (2) + 7 per bounce of its two sub-paths
+//   primary edge (2) + lens (2, with a lens only) + 7 per bounce of its two sub-paths
 RB_HD int secondary_edge_dim_base(const RenderParams& rp, int depth) {
     int off = 0;
     for (int d = rp.max_bounces - 1; d > depth; d--) off += 4 + 7 * (rp.max_bounces - 1 - d);
@@ -200,7 +202,7 @@ RB_HD int primary_edge_dim_base(const DevScene& sc, const RenderParams& rp) {
     return (sc.use_secondary_edge && sc.num_lights > 0) ? secondary_edge_dim_base(rp, -1) : 0;
 }
 RB_HD unsigned long long edge_draws_per_sample(const DevScene& sc, const RenderParams& rp) {
-    return (unsigned long long)(primary_edge_dim_base(sc, rp) + 2 + 7 * rp.max_bounces);
+    return (unsigned long long)(primary_edge_dim_base(sc, rp) + 2 + (RB_CAM_LENS(sc.cam) ? 2 : 0) + 7 * rp.max_bounces);
 }
 
 // Screen position of a pixel sample: consumes the first two sampler dimensions unless sample_pixel_center.  Under a pixel filter
@@ -219,12 +221,20 @@ RB_D void primary_sample_pos(const DevScene& sc, const RenderParams& rp, int px,
     sx = (double(px + sc.cam.vp_beg[0]) + jx) / double(sc.cam.width);
     sy = (double(py + sc.cam.vp_beg[1]) + jy) / double(sc.cam.height);
 }
+// Lens sample of a camera with a lens (the two sampler dimensions after the camera's), a point of the unit disc; (0, 0) without a lens.
+RB_D D2 primary_lens_sample(const DevScene& sc, Sampler& smp) {
+    if (!RB_CAM_LENS(sc.cam)) return d2(0, 0);
+    const double u1 = smp.next();
+    const double u2 = smp.next();
+    return concentric_disc(u1, u2);
+}
 // Camera sample -> primary ray (px, py are viewport-relative pixel coordinates), src/camera.cpp:8-43.
 RB_D void primary_ray_for(const DevScene& sc, const RenderParams& rp, int px, int py, Sampler& smp, double& sx, double& sy, Ray& ray, RayDiff& rd,
                           D3* org_d = nullptr, D3* dir_d = nullptr) {
     primary_sample_pos(sc, rp, px, py, smp, sx, sy);
-    cam_primary_ray(sc.cam, sx, sy, ray, rd);
-    if (org_d) cam_sample_primary(sc.cam, sx, sy, *org_d, *dir_d);
+    const D2 lu = primary_lens_sample(sc, smp);
+    cam_primary_ray(sc.cam, sx, sy, ray, rd, lu);
+    if (org_d) cam_sample_primary(sc.cam, sx, sy, *org_d, *dir_d, lu);
 }
 
 // Radiance of one pixel sample, already multiplied by 1/spp.
@@ -232,7 +242,7 @@ RB_D void primary_ray_for(const DevScene& sc, const RenderParams& rp, int px, in
 RB_D V3 forward_sample(const DevScene& sc, const RenderParams& rp, int pixel, int px, int py, int s, const unsigned long long* sobol = nullptr) {
     const Real weight = Real(1) / Real(rp.spp);
     Sampler smp;
-    smp.init(rp.sampler_type, rp.seed, pixel, (unsigned)s, sobol ? sobol : sc.sobol_matrices, RB_SOBOL_BITS, (unsigned long long)s * main_draws_per_sample(rp));
+    smp.init(rp.sampler_type, rp.seed, pixel, (unsigned)s, sobol ? sobol : sc.sobol_matrices, RB_SOBOL_BITS, (unsigned long long)s * main_draws_per_sample(sc, rp));
     double sx, sy;
     Ray ray;
     RayDiff rd;
@@ -354,7 +364,7 @@ RB_D void d_channel_values_at_hit(const DevScene& sc, const DevDScene& ds, const
 RB_D bool forward_sample_channels(const DevScene& sc, const RenderParams& rp, int pixel, int px, int py, int s, float* out, int* ids) {
     const Real weight = Real(1) / Real(rp.spp);
     Sampler smp;
-    smp.init(rp.sampler_type, rp.seed, pixel, (unsigned)s, sc.sobol_matrices, RB_SOBOL_BITS, (unsigned long long)s * main_draws_per_sample(rp));
+    smp.init(rp.sampler_type, rp.seed, pixel, (unsigned)s, sc.sobol_matrices, RB_SOBOL_BITS, (unsigned long long)s * main_draws_per_sample(sc, rp));
     double sx, sy;
     Ray ray;
     RayDiff rd;
@@ -418,7 +428,7 @@ RB_D int bwd_trace(const DevScene& sc, const RenderParams& rp, int pixel, int px
     Isect is = no_isect();
     RB_PHASE_SYNC();
     if (act) {
-        smp.init(rp.sampler_type, rp.seed, pixel, (unsigned)s, sc.sobol_matrices, RB_SOBOL_BITS, (unsigned long long)s * main_draws_per_sample(rp));
+        smp.init(rp.sampler_type, rp.seed, pixel, (unsigned)s, sc.sobol_matrices, RB_SOBOL_BITS, (unsigned long long)s * main_draws_per_sample(sc, rp));
         primary_ray_for(sc, rp, px, py, smp, sx, sy, ray, rd, &od, &dd);
         bool null_ray = ray_is_null(ray);
         act = !null_ray && closest_hit(sc, ray, is);
@@ -547,15 +557,16 @@ RB_D void bwd_sweep(const DevScene& sc, const KernelArgs& ka, int pixel, int px,
     d_ray.org += (d_prd.org_dx * (-psx) + d_prd.org_dy * (-psy)) / delta;
     d_ray.dir += (d_prd.dir_dx * (-psx) + d_prd.dir_dy * (-psy)) / delta;
     Sampler smp;
-    smp.init(rp.sampler_type, rp.seed, pixel, (unsigned)s, sc.sobol_matrices, RB_SOBOL_BITS, (unsigned long long)s * main_draws_per_sample(rp));
+    smp.init(rp.sampler_type, rp.seed, pixel, (unsigned)s, sc.sobol_matrices, RB_SOBOL_BITS, (unsigned long long)s * main_draws_per_sample(sc, rp));
     double sx, sy;
     primary_sample_pos(sc, rp, px, py, smp, sx, sy);
+    const D2 lu = primary_lens_sample(sc, smp);
     V2 d_screen = zero2();
     V2* d_screen_ptr = ka.screen_grad ? &d_screen : nullptr;
 #pragma unroll 1
     for (int k = 0; k < 3; k++) { // centre ray and its two offset rays; rolled to keep one copy of the camera adjoint
         DRay dr = k == 0 ? d_ray : k == 1 ? d_ray_dx : d_ray_dy;
-        d_cam_sample_primary(sc.cam, (Real)sx + (k == 1 ? delta : Real(0)), (Real)sy + (k == 2 ? delta : Real(0)), dr, cam_acc, d_screen_ptr);
+        d_cam_sample_primary(sc.cam, (Real)sx + (k == 1 ? delta : Real(0)), (Real)sy + (k == 2 ? delta : Real(0)), dr, cam_acc, d_screen_ptr, lu);
     }
     if (ka.screen_grad) {
         rb_red_add(&ka.screen_grad[2 * (size_t)pixel + 0], (float)d_screen.x);
@@ -709,7 +720,18 @@ struct PrimEdgePick {
     D2 q0, q1, ept;
     D2 upper, lower; // screen positions of the two rays on either side of the edge
     double jacobian; // 1 for linear projections (there the edge length and the gradient of the edge equation cancel)
+#ifndef RB_LEAN
+    D2 lu; // lens sample (unit disc) of a camera with a lens: the edge is projected from it, and both rays leave it
+#endif
 };
+// The lens sample of a pick; the lean kernels have no lens (RB_CAM_LENS is false there) and keep PrimEdgePick as it was without one.
+RB_D D2 pick_lens(const PrimEdgePick& pk) {
+#ifdef RB_LEAN
+    return d2(0, 0);
+#else
+    return pk.lu;
+#endif
+}
 // Gradients of the edge equation alpha(p) = dot(p, cross(v0_dir, v1_dir)) on the camera-space film w.r.t. the two projected
 // end points and the edge point (src/edge.cpp:737-757).
 RB_HD void primary_edge_grad_nonlinear(const DevCamera& cam, D2 q0, D2 q1, D2 ept, double* g) {
@@ -743,16 +765,63 @@ RB_HD bool primary_edge_pick_nonlinear(const DevScene& sc, V3 v0, V3 v1, PrimEdg
     pk.jacobian = line_jacobian * dirac_jacobian;
     return true;
 }
+// Ends of edge (v0, v1) projected from lens sample lu (lens_film_point in double), after the camera-space near clip of cam_project_d.
+RB_HD bool cam_project_lens_d(const DevCamera& cam, D3 p0, D3 p1, D2 lu, D2& q0, D2& q1) {
+    D3 a = w2c_point(cam, p0), b = w2c_point(cam, p1);
+    double cn = cam.clip_near;
+    if (a.z < cn && b.z < cn) return false;
+    if (a.z < cn) {
+        D3 dir = d3(a.x - b.x, a.y - b.y, a.z - b.z);
+        double t = -(b.z - cn) / dir.z;
+        a = d3(b.x + t * dir.x, b.y + t * dir.y, b.z + t * dir.z);
+    } else if (b.z < cn) {
+        D3 dir = d3(b.x - a.x, b.y - a.y, b.z - a.z);
+        double t = -(a.z - cn) / dir.z;
+        b = d3(a.x + t * dir.x, a.y + t * dir.y, a.z + t * dir.z);
+    }
+    const double f = cam.focus_distance, lx = cam.lens_radius * lu.x, ly = cam.lens_radius * lu.y;
+    q0 = cam_to_screen_d(cam, d3(lx / f + (a.x - lx) / a.z, ly / f + (a.y - ly) / a.z, 1.0));
+    q1 = cam_to_screen_d(cam, d3(lx / f + (b.x - lx) / b.z, ly / f + (b.y - ly) / b.z, 1.0));
+    return true;
+}
+// The lens camera's pick: the edge projected from the lens point, a uniform point on the projected segment, dropped when it is off
+// screen or when the edge is no silhouette seen from the lens point.  The projection is linear, so the pinhole's offsets and jacobian
+// carry over.
+RB_D bool primary_edge_pick_lens(const DevScene& sc, const Edge& edge, V3 v0, V3 v1, D2 lu, PrimEdgePick& pk) {
+    if (pk.pmf <= 0) return false;
+    if (!cam_project_lens_d(sc.cam, d3(v0.x, v0.y, v0.z), d3(v1.x, v1.y, v1.z), lu, pk.q0, pk.q1)) return false;
+    pk.ept.x = pk.q0.x + pk.e_t * (pk.q1.x - pk.q0.x);
+    pk.ept.y = pk.q0.y + pk.e_t * (pk.q1.y - pk.q0.y);
+    if (!cam_in_screen(sc.cam, mk2((Real)pk.ept.x, (Real)pk.ept.y))) return false;
+    const double* C = sc.cam.c2w;
+    const double lx = sc.cam.lens_radius * lu.x, ly = sc.cam.lens_radius * lu.y, iw = 1.0 / (C[12] * lx + C[13] * ly + C[15]);
+    const V3 lens_world = mk3((Real)((C[0] * lx + C[1] * ly + C[3]) * iw), (Real)((C[4] * lx + C[5] * ly + C[7]) * iw), (Real)((C[8] * lx + C[9] * ly + C[11]) * iw));
+    if (!edge_is_silhouette(sc.shapes, lens_world, edge)) return false;
+    double ddx = pk.q0.x - pk.q1.x, ddy = pk.q0.y - pk.q1.y;
+    double dl = sqrt(ddx * ddx + ddy * ddy);
+    double nx = ddy / dl, ny = -ddx / dl;
+    const double offset = 1e-6;
+    pk.upper.x = pk.ept.x + nx * offset;
+    pk.upper.y = pk.ept.y + ny * offset;
+    pk.lower.x = pk.ept.x - nx * offset;
+    pk.lower.y = pk.ept.y - ny * offset;
+    pk.jacobian = 1;
+    return true;
+}
 RB_D bool primary_edge_pick(const DevScene& sc, const RenderParams& rp, long long i, int s, int dim_base, Sampler& smp, PrimEdgePick& pk) {
     smp.init(rp.sampler_type, rp.seed + 131071ULL, (int)i, (unsigned)s, sc.sobol_matrices, RB_SOBOL_BITS,
              (unsigned long long)s * edge_draws_per_sample(sc, rp));
     smp.skip(dim_base);
     double e_sel = smp.next();
     pk.e_t = smp.next();
+#ifndef RB_LEAN
+    pk.lu = primary_lens_sample(sc, smp);
+#endif
     pk.edge_id = cdf_pick(sc.prim_edge_cdf, sc.num_edges, e_sel);
     pk.pmf = sc.prim_edge_pmf[pk.edge_id];
     const Edge edge = sc.edges[pk.edge_id];
     V3 v0 = edge_v0(sc.shapes, edge), v1 = edge_v1(sc.shapes, edge);
+    if (RB_CAM_LENS(sc.cam)) return primary_edge_pick_lens(sc, edge, v0, v1, pick_lens(pk), pk);
     if (!cam_project_d(sc.cam, d3(v0.x, v0.y, v0.z), d3(v1.x, v1.y, v1.z), pk.q0, pk.q1)) return false;
     if (pk.pmf <= 0) return false;
     if (cam_is_linear(sc.cam)) {
@@ -845,6 +914,7 @@ RB_D void primary_edge_sample(const DevScene& sc, const KernelArgs& ka, long lon
     Sampler smp;
     PrimEdgePick pk;
     if (!primary_edge_pick(sc, rp, i, s, dim_base, smp, pk)) return;
+    const D2 lu = pick_lens(pk);
     if (ka.zero_cull && edge_point_adjoint_is_zero(sc, ka, pk.ept)) return; // (before any ray: k_prim_keys drops these samples too)
     const double pmf = pk.pmf;
     const D2 q0 = pk.q0, q1 = pk.q1, ept = pk.ept;
@@ -867,14 +937,14 @@ RB_D void primary_edge_sample(const DevScene& sc, const KernelArgs& ka, long lon
     // ray differential of the un-offset ray, shared by both sides (src/edge.cpp:594-608)
     Ray cray;
     RayDiff rd;
-    cam_primary_ray(sc.cam, ept.x, ept.y, cray, rd);
+    cam_primary_ray(sc.cam, ept.x, ept.y, cray, rd, lu);
     Real contrib = 0;
     Ray rays[2];
     Isect hits[2];
     bool connected = false;
     for (int side = 0; side < 2; side++) {
         D3 o, d;
-        cam_sample_primary(sc.cam, side == 0 ? pk.upper.x : pk.lower.x, side == 0 ? pk.upper.y : pk.lower.y, o, d);
+        cam_sample_primary(sc.cam, side == 0 ? pk.upper.x : pk.lower.x, side == 0 ? pk.upper.y : pk.lower.y, o, d, lu);
         rays[side] = make_ray(o, d);
         hits[side] = no_isect();
         if (!ray_is_null(rays[side])) closest_hit(sc, rays[side], hits[side]);
@@ -932,7 +1002,8 @@ RB_D void primary_edge_sample(const DevScene& sc, const KernelArgs& ka, long lon
         dex = (Real)g[4] * contrib; dey = (Real)g[5] * contrib;
     }
     V3 d_v0 = zero3(), d_v1 = zero3();
-    d_cam_project(sc.cam, v0, v1, d0x, d0y, d1x, d1y, cam_acc, d_v0, d_v1);
+    if (RB_CAM_LENS(sc.cam)) d_cam_project_lens(sc.cam, v0, v1, lu, d0x, d0y, d1x, d1y, cam_acc, d_v0, d_v1);
+    else d_cam_project(sc.cam, v0, v1, d0x, d0y, d1x, d1y, cam_acc, d_v0, d_v1);
     float* dv = ds.shapes[edge.shape_id].vertices;
     if (dv) {
         agg_add3(dv + 3 * (size_t)edge.v0, d_v0);
@@ -991,4 +1062,6 @@ RB_HD void finish_camera(const DevCamera& cam, const double* acc, const rb_dcame
         for (int k = 0; k < 9; k++) out.intrinsic_mat[k] += (float)acc[41 + k];
     if (out.distortion)
         for (int k = 0; k < 8; k++) out.distortion[k] += (float)acc[50 + k];
+    if (out.lens && cam.lens_radius > 0)
+        for (int k = 0; k < 2; k++) out.lens[k] += (float)acc[RB_CAM_ACC + k];
 }

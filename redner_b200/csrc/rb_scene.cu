@@ -769,7 +769,7 @@ extern "C" int rb_scene_set_camera(rb_scene* sc, const rb_camera* cam) {
         rb_set_error("rb_scene_set_camera: the scene's last update failed; update it again or build a new scene");
         return 1;
     }
-    if (const char* err = host_check_filter_camera(rb_pixel_filter{sc->dev.cam.filter_type, sc->dev.cam.filter_width}, *cam)) {
+    if (const char* err = host_check_camera(rb_pixel_filter{sc->dev.cam.filter_type, sc->dev.cam.filter_width}, *cam)) {
         rb_set_error(err);
         retitle_error("rb_scene_set_camera");
         return 1;

@@ -38,17 +38,27 @@ inline rb_pixel_filter host_pixel_filter(const rb_pixel_filter& f) {
     return f;
 }
 inline bool host_pixel_box(const rb_pixel_filter& f) { return f.type == RB_FILTER_BOX && f.width == 1.f; }
-// A camera the primary-edge pass of a pixel filter other than the 1-pixel box handles: linear projection, no lens model.
-inline const char* host_check_filter_camera(const rb_pixel_filter& f, const rb_camera& cam) {
+// The camera against the scene's pixel filter: a filter other than the 1-pixel box needs a linear projection without a lens model, and a
+// thin lens (rb_camera::lens_radius > 0) a perspective camera without distortion, with the 1-pixel box and an intrinsic matrix whose
+// last row is (0, 0, k) (the primary-edge distribution bounds the circle of confusion through it).
+inline const char* host_check_camera(const rb_pixel_filter& f, const rb_camera& cam) {
     if (!host_pixel_box(host_pixel_filter(f)) && (cam.camera_type == RB_CAMERA_FISHEYE || cam.camera_type == RB_CAMERA_PANORAMA || cam.has_distortion))
         return "rb_scene_create: pixel filters other than the 1-pixel box need a perspective or orthographic camera without lens distortion";
+    if (!(std::isfinite(cam.lens_radius) && cam.lens_radius >= 0.f)) return "rb_scene_create: the lens_radius of a thin lens must be finite and >= 0";
+    if (cam.lens_radius == 0.f) return nullptr;
+    if (!(std::isfinite(cam.focus_distance) && cam.focus_distance > 0.f)) return "rb_scene_create: the focus_distance of a thin lens must be finite and > 0";
+    if (cam.camera_type != RB_CAMERA_PERSPECTIVE) return "rb_scene_create: a thin lens (lens_radius > 0) needs a perspective camera";
+    if (cam.has_distortion) return "rb_scene_create: a thin lens (lens_radius > 0) cannot be combined with a distortion model";
+    if (!host_pixel_box(host_pixel_filter(f))) return "rb_scene_create: a thin lens (lens_radius > 0) needs the 1-pixel box pixel filter";
+    if (cam.intrinsic_mat[6] != 0.f || cam.intrinsic_mat[7] != 0.f || cam.intrinsic_mat[8] == 0.f)
+        return "rb_scene_create: a thin lens (lens_radius > 0) needs an intrinsic_mat whose last row is (0, 0, k) with k != 0";
     return nullptr;
 }
 inline const char* host_check_pixel_filter(const rb_scene_desc& desc) {
     const rb_pixel_filter f = host_pixel_filter(desc.pixel_filter);
     if (f.type != RB_FILTER_BOX && f.type != RB_FILTER_TENT && f.type != RB_FILTER_GAUSSIAN) return "rb_scene_create: unknown pixel filter type";
     if (!(f.width > 0.f && f.width <= 4.f)) return "rb_scene_create: pixel filter width must lie in (0, 4] pixels";
-    return host_check_filter_camera(f, desc.camera);
+    return host_check_camera(f, desc.camera);
 }
 inline void host_setup_pixel_filter(const rb_pixel_filter& f, DevCamera& dc) {
     const rb_pixel_filter g = host_pixel_filter(f);
@@ -599,6 +609,8 @@ inline void host_setup_camera(const rb_camera& c, DevCamera& dc) {
     dc.vp_beg[1] = c.viewport_beg[1];
     dc.vp_end[0] = c.viewport_end[0];
     dc.vp_end[1] = c.viewport_end[1];
+    dc.lens_radius = c.lens_radius > 0.f ? c.lens_radius : 0.f;
+    dc.focus_distance = c.lens_radius > 0.f ? c.focus_distance : 0.f;
 }
 // compute_num_channels, src/channels.cpp:42-113
 inline int host_compute_num_channels(const int* channels, int n, int max_generic) {

@@ -60,6 +60,9 @@ RB_HD SurfacePoint zero_point() {
 struct DevCamera {
     int width, height;
     int use_look_at;
+    // thin lens (rb_camera::lens_radius / focus_distance); lens_radius == 0: the pinhole, focus_distance is then 0 as well.  The two floats
+    // sit in what was alignment padding, so that DevCamera, and the kernels' parameter layout behind it, keep their size and offsets.
+    float lens_radius;
     double position[3], look[3], up[3];
     double c2w[16], w2c[16];
     double intr_inv[9], intr[9];
@@ -67,6 +70,7 @@ struct DevCamera {
     int type;
     int vp_beg[2], vp_end[2];
     int has_distortion;   // Brown-Conrady lens model, src/camera_distortion.h
+    float focus_distance; // (thin lens, see lens_radius)
     double distortion[8]; // k1..k6 (radial, rational), p1, p2 (tangential)
     // the scene's pixel filter (rb_scene_desc::pixel_filter, { 0, 0 } made { RB_FILTER_BOX, 1 }); rb_scene_set_camera keeps it
     int filter_type;
@@ -173,7 +177,7 @@ struct DevDScene {
     rb_texture env_values; // gradient mip pyramid of the environment map (num_levels == 0: none)
     float* env_w2e;        // 16 floats, gradient of world_to_env
     // internal double accumulators for the camera (reduced per block, finished by one tiny kernel):
-    // [0..15] d_cam_to_world, [16..31] d_world_to_cam, [32..40] d_intrinsic_mat_inv, [41..49] d_intrinsic_mat
+    // [0..15] d_cam_to_world, [16..31] d_world_to_cam, [32..40] d_intrinsic_mat_inv, [41..49] d_intrinsic_mat, ... (CamAcc, rb_camera.cuh)
     double* cam_accum;
 };
 

@@ -79,7 +79,8 @@ class Vector2i:  # src/redner.cpp:218-221
 
 class Camera:  # src/redner.cpp:34-50, src/camera.h:22-66
     def __init__(self, width, height, position, look, up, cam_to_world, world_to_cam, intrinsic_mat_inv, intrinsic_mat,
-                 distortion_params, clip_near, camera_type, viewport_beg, viewport_end):
+                 distortion_params, clip_near, camera_type, viewport_beg, viewport_end, lens_radius=0.0, focus_distance=1.0):
+        """`lens_radius`, `focus_distance` (redner_b200 extension): a thin lens, in world units; lens_radius 0 is the pinhole."""
         c = L.rb_camera()
         c.width, c.height = int(width), int(height)
         c2w = _read_floats(cam_to_world, 16)
@@ -103,6 +104,7 @@ class Camera:  # src/redner.cpp:34-50, src/camera.h:22-66
         c.camera_type = int(camera_type)
         c.viewport_beg[:] = [viewport_beg.x, viewport_beg.y]
         c.viewport_end[:] = [viewport_end.x, viewport_end.y]
+        c.lens_radius, c.focus_distance = float(lens_radius), float(focus_distance)
         self._c = c
         self.use_look_at = bool(c.use_look_at)
 
@@ -111,12 +113,14 @@ class Camera:  # src/redner.cpp:34-50, src/camera.h:22-66
 
 
 class DCamera:  # src/redner.cpp:52-60
-    def __init__(self, position, look, up, cam_to_world, world_to_cam, intrinsic_mat_inv, intrinsic_mat, distortion_params):
+    def __init__(self, position, look, up, cam_to_world, world_to_cam, intrinsic_mat_inv, intrinsic_mat, distortion_params, lens=None):
+        """`lens` (redner_b200 extension): 2 floats receiving d(lens_radius), d(focus_distance), or None."""
         d = L.rb_dcamera()
         d.position, d.look, d.up = _addr(position) or None, _addr(look) or None, _addr(up) or None
         d.cam_to_world, d.world_to_cam = _addr(cam_to_world) or None, _addr(world_to_cam) or None
         d.intrinsic_mat_inv, d.intrinsic_mat = _addr(intrinsic_mat_inv) or None, _addr(intrinsic_mat) or None
         d.distortion = _addr(distortion_params) or None
+        d.lens = _addr(lens) or None
         self._c = d
 
 

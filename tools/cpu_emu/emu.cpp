@@ -377,7 +377,7 @@ extern "C" int rb_scene_edge_list(const rb_scene* sc, int* num_edges, int* edges
 // builders; geometry, BVH, lights and the edge list are kept (mirrors rb_scene_set_camera of the product, which rebuilds them on the GPU).
 extern "C" int rb_scene_set_camera(rb_scene* sc, const rb_camera* cam) {
     DevScene& d = sc->dev;
-    if (const char* err = host_check_filter_camera(rb_pixel_filter{d.cam.filter_type, d.cam.filter_width}, *cam)) {
+    if (const char* err = host_check_camera(rb_pixel_filter{d.cam.filter_type, d.cam.filter_width}, *cam)) {
         g_err = std::string("rb_scene_set_camera:") + (err + 16);
         return 1;
     }
@@ -460,6 +460,10 @@ static int emu_render(const rb_scene* scene, const rb_options* opt, float* image
         g_err = "rb_render: this build has no GGX specular lobe (specular_model)";
         return 1;
     }
+    if (scene->dev.cam.lens_radius > 0) {
+        g_err = "rb_render: this build has no thin lens (lens_radius)";
+        return 1;
+    }
 #endif
     const DevScene& sc = scene->dev;
     if (image && !rp.only_radiance) {
@@ -489,8 +493,9 @@ static int emu_render(const rb_scene* scene, const rb_options* opt, float* image
             g_err = err;
             return 1;
         }
-        std::vector<double> cam_accum(RB_CAM_ACC, 0.0);
-        std::vector<float> cam_f(RB_CAM_ACC, 0.f);
+        const int n_cam = cam_acc_count(sc.cam);
+        std::vector<double> cam_accum(n_cam, 0.0);
+        std::vector<float> cam_f(n_cam, 0.f);
         ka.ds.shapes = d_scene->shapes;
         ka.ds.materials = d_scene->materials;
         ka.ds.light_intensity = d_scene->light_intensity;
@@ -554,7 +559,7 @@ static int emu_render(const rb_scene* scene, const rb_options* opt, float* image
                     rb_emu_rank = &ranks[((size_t)s * npx + (size_t)y * rp.vp_w + x) * mbr];
 #endif
                     backward_sample(sc, ka, y * rp.vp_w + x, x, y, s, recs.data(), acc);
-                    for (int k = 0; k < RB_CAM_ACC; k++) { cam_accum[k] += cam_f[k]; cam_f[k] = 0.f; }
+                    for (int k = 0; k < n_cam; k++) { cam_accum[k] += cam_f[k]; cam_f[k] = 0.f; }
                     exact_sample_done();
                 }
         if (primary_edge_pass_runs(sc)) {
@@ -563,18 +568,18 @@ static int emu_render(const rb_scene* scene, const rb_options* opt, float* image
                 for (int s = 0; s < rp.spp; s++) {
                     if (i % rp.num_parts != rp.part) continue; // primary-edge samples are sharded by sample index
                     primary_edge_sample(sc, ka, i, s, primary_edge_dim_base(sc, rp), acc);
-                    for (int k = 0; k < RB_CAM_ACC; k++) { cam_accum[k] += cam_f[k]; cam_f[k] = 0.f; }
+                    for (int k = 0; k < n_cam; k++) { cam_accum[k] += cam_f[k]; cam_f[k] = 0.f; }
                     exact_sample_done();
                 }
         }
         if (records) {
             for (long long i = 0; i < xl.num_acc; i++)
                 exact_export(&xacc[(size_t)i * RB_EXACT_WORDS],
-                             records + exact_record_of(i, xl.ranges.data(), xl.rec_first.data(), (int)xl.ranges.size(), RB_CAM_ACC) * RB_EXACT_RECORD_WORDS);
+                             records + exact_record_of(i, xl.ranges.data(), xl.rec_first.data(), (int)xl.ranges.size(), n_cam) * RB_EXACT_RECORD_WORDS);
             return 0;
         }
         if (det)
-            for (long long i = 0; i < xl.num_acc; i++) exact_finalise(xacc.data(), i, xl.ranges.data(), (int)xl.ranges.size(), cam_accum.data(), RB_CAM_ACC);
+            for (long long i = 0; i < xl.num_acc; i++) exact_finalise(xacc.data(), i, xl.ranges.data(), (int)xl.ranges.size(), cam_accum.data(), n_cam);
         finish_camera(sc.cam, cam_accum.data(), d_scene->camera);
     }
     return 0;
@@ -633,11 +638,12 @@ extern "C" int rb_exact_round(const rb_scene* scene, const rb_options* opt, cons
         return 1;
     }
     std::vector<long long> acc((size_t)(xl.num_acc + 1) * RB_EXACT_WORDS, 0);
-    std::vector<double> cam_accum(RB_CAM_ACC, 0.0);
+    const int n_cam = cam_acc_count(scene->dev.cam);
+    std::vector<double> cam_accum(n_cam, 0.0);
     for (long long i = 0; i < xl.num_acc; i++)
-        exact_import(records + exact_record_of(i, xl.ranges.data(), xl.rec_first.data(), (int)xl.ranges.size(), RB_CAM_ACC) * RB_EXACT_RECORD_WORDS,
+        exact_import(records + exact_record_of(i, xl.ranges.data(), xl.rec_first.data(), (int)xl.ranges.size(), n_cam) * RB_EXACT_RECORD_WORDS,
                      &acc[(size_t)i * RB_EXACT_WORDS]);
-    for (long long i = 0; i < xl.num_acc; i++) exact_finalise(acc.data(), i, xl.ranges.data(), (int)xl.ranges.size(), cam_accum.data(), RB_CAM_ACC);
+    for (long long i = 0; i < xl.num_acc; i++) exact_finalise(acc.data(), i, xl.ranges.data(), (int)xl.ranges.size(), cam_accum.data(), n_cam);
     finish_camera(scene->dev.cam, cam_accum.data(), d_scene->camera);
     return 0;
 }
