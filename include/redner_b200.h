@@ -289,6 +289,10 @@ int rb_scene_last_stage_stats(const rb_scene* scene, float* stage_ms4, double* p
 /* Split of the backward bands of the last rb_render, summed over the bands:
  * { k_bwd_trace, scan + compaction + k_bwd_secondary, k_bwd_sweep } in milliseconds. */
 int rb_scene_last_backward_stats(const rb_scene* scene, float* bwd_ms3);
+/* Work of the backward bands of the last rb_render: the samples of the owned pixels whose d_rendered_image is not exactly zero in
+ * every float (every owned sample with RB_NO_ZERO_CULL=1), which are the only ones the bands run over, and the number of bands they
+ * took.  Both are 0 after a call without d_rendered_image. */
+int rb_scene_last_live_samples(const rb_scene* scene, long long* live_samples, long long* num_bands);
 /* Bytes of exact gradient accumulators (rb_options::deterministic) the last rb_render on this scene took from the backward scratch:
  * 88 per accumulator, one per camera scalar and per float of the gradient buffers (overlapping buffers share them), plus a spare;
  * 0 when the last call was not a deterministic backward pass. */

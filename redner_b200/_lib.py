@@ -133,7 +133,7 @@ class rb_dscene_desc(C.Structure):
 
 EXPORTS = [
     "rb_scene_create", "rb_scene_create_on_stream", "rb_scene_destroy", "rb_scene_max_generic_texture_dimension", "rb_compute_num_channels", "rb_render",
-    "rb_scene_set_partition", "rb_scene_last_stats", "rb_scene_last_stage_stats", "rb_scene_last_backward_stats", "rb_scene_last_exact_bytes", "rb_release_scratch", "rb_scene_build_ms", "rb_scene_edge_trees", "rb_scene_edge_list", "rb_scene_table", "rb_scene_trace_rays", "rb_exact_sum_test", "rb_texture_test", "rb_envmap_test", "rb_scene_set_camera", "rb_scene_update", "rb_render_batch", "rb_exact_record_count", "rb_render_exact", "rb_exact_round", "rb_last_error", "rb_version",
+    "rb_scene_set_partition", "rb_scene_last_stats", "rb_scene_last_stage_stats", "rb_scene_last_backward_stats", "rb_scene_last_live_samples", "rb_scene_last_exact_bytes", "rb_release_scratch", "rb_scene_build_ms", "rb_scene_edge_trees", "rb_scene_edge_list", "rb_scene_table", "rb_scene_trace_rays", "rb_exact_sum_test", "rb_texture_test", "rb_envmap_test", "rb_scene_set_camera", "rb_scene_update", "rb_render_batch", "rb_exact_record_count", "rb_render_exact", "rb_exact_round", "rb_last_error", "rb_version",
 ]
 
 
@@ -166,6 +166,9 @@ def _bind(lib):
     if hasattr(lib, "rb_scene_last_backward_stats"):
         lib.rb_scene_last_backward_stats.argtypes = [C.c_void_p, c_float_p]
         lib.rb_scene_last_backward_stats.restype = C.c_int
+    if hasattr(lib, "rb_scene_last_live_samples"):
+        lib.rb_scene_last_live_samples.argtypes = [C.c_void_p, C.POINTER(C.c_longlong), C.POINTER(C.c_longlong)]
+        lib.rb_scene_last_live_samples.restype = C.c_int
     if hasattr(lib, "rb_scene_last_exact_bytes"):
         lib.rb_scene_last_exact_bytes.argtypes = [C.c_void_p, C.POINTER(C.c_size_t)]
         lib.rb_scene_last_exact_bytes.restype = C.c_int

@@ -17,6 +17,7 @@
 
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
+#include <cub/device/device_select.cuh>
 #include <thrust/iterator/counting_iterator.h>
 #include <thrust/iterator/transform_iterator.h>
 
@@ -98,6 +99,20 @@ static int pick_grid(const void* kernel, int device, int block = RB_BLOCK, size_
 enum { EV_BEGIN, EV_AFTER_FORWARD, EV_AFTER_BANDS, EV_AFTER_PRIMARY_EDGE, EV_END, NUM_FIXED_EVENTS };
 enum { BAND_BEGIN, BAND_AFTER_TRACE, BAND_BEFORE_SWEEP, BAND_END, BAND_EVENTS };
 
+// Live-pixel list of a backward pass (KernelArgs::live_pixels): owned pixel k, row-major over the owned rows, -> its viewport pixel, kept
+// by cub::DeviceSelect::If when its adjoint is not zero.  The selection keeps the input order, so the list is ascending.
+struct OwnedPixelOf {
+    RenderParams rp;
+    __host__ __device__ int operator()(int k) const {
+        int j = k / rp.vp_w;
+        return owned_row_to_row(rp, j) * rp.vp_w + (k - j * rp.vp_w);
+    }
+};
+struct PixelIsLive {
+    KernelArgs ka;
+    __host__ __device__ bool operator()(int pixel) const { return !ka.zero_cull || !pixel_adjoint_is_zero(ka, pixel); }
+};
+
 // The caller's records of rb_render_exact: the backward pass ends by adding its accumulators into them instead of rounding.
 struct ExactExport {
     long long* records;
@@ -163,6 +178,7 @@ static int render_pass(const rb_scene* scene_, const rb_options* opt, float* ima
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, scene->device);
     std::vector<BandCounters> host_counters;
     long long num_bands_done = 0;
+    long long live_samples = 0; // samples of the pixels whose adjoint is not zero (backward)
     size_t exact_bytes = 0; // exact accumulators of a deterministic backward pass
     std::unique_lock<std::mutex> scratch_lock; // per-device scratch, held for the backward pass (released before the guard runs)
     void* args[] = {&scene->dev, &ka}; // parameters of every kernel in `kern` but the primary-edge pair (read at each launch)
@@ -211,7 +227,8 @@ static int render_pass(const rb_scene* scene_, const rb_options* opt, float* ima
             return 1;
         }
         const bool secondary = boundary_stage_runs(scene->dev, rp);
-        const long long total_samples = (long long)ka.owned_rows * rp.vp_w * rp.spp;
+        const int owned_px = ka.owned_rows * rp.vp_w;
+        const long long total_samples = (long long)owned_px * rp.spp; // (the bands run over the live ones only; this bounds their number)
         ka.rec_per_sample = rp.max_bounces + 1;
         const size_t per_sample = (size_t)ka.rec_per_sample * (sizeof(VertexRec) + (secondary ? sizeof(V3) + sizeof(EdgePick) + 16 : 0)) + 2 * sizeof(int) +
                                   sizeof(ListCount) + (secondary ? sizeof(ulonglong2) : 0);
@@ -224,11 +241,10 @@ static int render_pass(const rb_scene* scene_, const rb_options* opt, float* ima
         band = std::min<long long>(band, (1LL << 30) / ka.rec_per_sample);
         if (det) band = std::min(band, exact_max_samples);
         band = std::min<long long>(band, std::max<long long>(total_samples, 1));
-        const long long num_bands = (total_samples + band - 1) / band;
-        if (!events.ensure((size_t)(NUM_FIXED_EVENTS + BAND_EVENTS * num_bands))) {
-            rb_set_error("rb_render: cudaEventCreate failed");
-            return 1;
-        }
+        const long long max_bands = (total_samples + band - 1) / band;
+        auto owned_it = thrust::make_transform_iterator(thrust::counting_iterator<int>(0), OwnedPixelOf{rp});
+        size_t select_bytes = 0;
+        cub::DeviceSelect::If(nullptr, select_bytes, owned_it, (int*)nullptr, (int*)nullptr, owned_px, PixelIsLive{ka}, stream);
         auto count_it = thrust::make_transform_iterator(thrust::counting_iterator<int>(0), ListCountOf{nullptr, nullptr});
         size_t scan_bytes = 0;
         cub::DeviceScan::ExclusiveScan(nullptr, scan_bytes, count_it, (ListCount*)nullptr, ListCountSum(), ListCount{0, 0, 0, 0}, (int)band, stream);
@@ -243,7 +259,8 @@ static int render_pass(const rb_scene* scene_, const rb_options* opt, float* ima
         cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, (const unsigned*)nullptr, (unsigned*)nullptr, (const unsigned*)nullptr, (unsigned*)nullptr, (int)band_e, 0, 32, stream);
 
         // ---- scratch layout, in carving order, every buffer 256-byte aligned: gradient descriptors | camera accumulators | band counters |
-        //      edge histogram, offsets and cursors | band (records, boundary terms, work lists).  The primary-edge pass runs after the
+        //      edge histogram, offsets and cursors | live-pixel list, its count and its selection temporaries | band (records, boundary
+        //      terms, work lists).  The primary-edge pass runs after the
         //      bands and reuses the band area for its keys / values (double buffers) and radix-sort temporaries.  The buffers of the
         //      boundary stage are empty when it does not run.  carve(nullptr) only measures; both calls return the size.
         rb_dshape* d_shapes;
@@ -255,7 +272,8 @@ static int render_pass(const rb_scene* scene_, const rb_options* opt, float* ima
         long long* exact_acc; // deterministic mode: xl.num_acc accumulators and the spare
         ExactRange* exact_ranges;
         long long* exact_rec_first; // (rb_render_exact)
-        void *scan_tmp, *sort_tmp;
+        int *live_pixels, *live_count;
+        void *select_tmp, *scan_tmp, *sort_tmp;
         unsigned *k0, *k1, *v0, *v1;
         size_t zeroed_bytes = 0;
         auto carve = [&](char* base) {
@@ -275,11 +293,14 @@ static int render_pass(const rb_scene* scene_, const rb_options* opt, float* ima
             // Every pass starts with these three at zero.  They stay adjacent, carved one after the other, so that one memset clears them.
             const size_t zeroed_begin = off;
             cam_accum = (double*)take(RB_CAM_ACC_LENS * sizeof(double));
-            counters = (BandCounters*)take((size_t)num_bands * sizeof(BandCounters));
+            counters = (BandCounters*)take((size_t)max_bands * sizeof(BandCounters));
             ka.edge_hist = (unsigned*)take(secondary ? n_edges * 4 : 0);
             zeroed_bytes = off - zeroed_begin;
             ka.edge_offs = (unsigned*)take(secondary ? n_edges * 4 : 0);
             ka.edge_cursor = (unsigned*)take(secondary ? n_edges * 4 : 0);
+            live_pixels = (int*)take((size_t)owned_px * sizeof(int));
+            live_count = (int*)take(sizeof(int));
+            select_tmp = take(select_bytes);
             const size_t band_begin = off;
             ka.records = (VertexRec*)take(n_rec * sizeof(VertexRec));
             V3* dpos = (V3*)take(secondary ? n_rec * sizeof(V3) : 0);
@@ -340,16 +361,30 @@ static int render_pass(const rb_scene* scene_, const rb_options* opt, float* ima
         ka.ds.light_intensity = d_lights;
         ka.ds.cam_accum = cam_accum;
 
+        // ---- the live pixels: those of the owned rows whose adjoint is not zero, in ascending order.  Their count is the one value
+        //      read back inside the pass: the bands then cover the live samples only, so a mostly-zero adjoint runs few bands.
+        ka.live_pixels = live_pixels;
+        RB_CUDA_OK(cub::DeviceSelect::If(select_tmp, select_bytes, owned_it, live_pixels, live_count, owned_px, PixelIsLive{ka}, stream));
+        launches += 2;
+        int n_live_px = 0;
+        RB_CUDA_OK(cudaMemcpyAsync(&n_live_px, live_count, sizeof(int), cudaMemcpyDeviceToHost, stream));
+        RB_CUDA_OK(cudaStreamSynchronize(stream));
+        live_samples = (long long)n_live_px * rp.spp;
+        if (!events.ensure((size_t)(NUM_FIXED_EVENTS + BAND_EVENTS * ((live_samples + band - 1) / band)))) {
+            rb_set_error("rb_render: cudaEventCreate failed");
+            return 1;
+        }
+
         // ---- interior + first-hit adjoints, band by band: trace (+ work lists) -> boundary terms (pick, counting sort by edge, shade)
-        //      -> sweep.  Every list size stays on the device: fixed persistent grids, no host synchronisation inside the pass.
+        //      -> sweep.  Every list size stays on the device: fixed persistent grids, no host synchronisation inside the bands.
         const int grid_t = pick_grid(bkern.bwd_trace, scene->device, RB_BLOCK_TRACE);
         const int grid_p = pick_grid(bkern.bwd_sec_pick, scene->device, RB_BLOCK_SEC);
         const int grid_s = pick_grid(bkern.bwd_sec_shade, scene->device, RB_BLOCK_SEC);
         const int grid_w = pick_grid(bkern.bwd_sweep, scene->device, RB_BLOCK_SWEEP, cam_smem_sweep);
         long long band_idx = 0;
-        for (long long i0 = 0; i0 < total_samples; i0 += band, band_idx++) {
+        for (long long i0 = 0; i0 < live_samples; i0 += band, band_idx++) {
             ka.band_i0 = i0;
-            ka.band_n = (int)std::min<long long>(band, total_samples - i0);
+            ka.band_n = (int)std::min<long long>(band, live_samples - i0);
             ka.counters = counters + band_idx;
             cudaEvent_t* bev = &ev[(size_t)(NUM_FIXED_EVENTS + BAND_EVENTS * band_idx)];
             RB_CUDA_OK(cudaEventRecord(bev[BAND_BEGIN], stream));
@@ -428,6 +463,8 @@ static int render_pass(const rb_scene* scene_, const rb_options* opt, float* ima
     float ms = 0.f;
     cudaEventElapsedTime(&ms, ev[EV_BEGIN], ev[EV_END]);
     scene->last_launches = launches;
+    scene->last_live_samples = live_samples;
+    scene->last_bands = num_bands_done;
     scene->last_exact_bytes = exact_bytes;
     scene->last_kernel_ms = ms;
     for (int i = EV_BEGIN; i < EV_END; i++) { // k_forward, backward bands, primary edges, k_finish_camera

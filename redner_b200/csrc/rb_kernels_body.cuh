@@ -193,18 +193,18 @@ RB_D void exact_camera_flush(long long* cam_exact, int n_cam) {
 }
 #endif
 
-// Dense sample index of the band -> (pixel, px, py, s).  Consecutive lanes are consecutive samples of a pixel.
+// Dense live sample index -> (pixel, px, py, s): sample s of live pixel I / spp.  Consecutive lanes are consecutive samples of a pixel.
 struct SampleId {
     int pixel, px, py, s;
 };
-RB_D SampleId band_sample(const RenderParams& rp, long long I) {
+RB_D SampleId band_sample(const KernelArgs& ka, long long I) {
+    const RenderParams& rp = ka.rp;
     long long k = I / rp.spp;
     SampleId id;
     id.s = (int)(I - k * rp.spp);
-    int j = (int)(k / rp.vp_w);
-    id.px = (int)(k - (long long)j * rp.vp_w);
-    id.py = owned_row_to_row(rp, j);
-    id.pixel = id.py * rp.vp_w + id.px;
+    id.pixel = ka.live_pixels[k];
+    id.py = id.pixel / rp.vp_w;
+    id.px = id.pixel - id.py * rp.vp_w;
     return id;
 }
 // The work loops below are BLOCK-uniform (every thread of a block runs the same number of iterations, idle ones with
@@ -216,16 +216,15 @@ RB_D SampleId band_sample(const RenderParams& rp, long long I) {
 // boundary stage will look at it at all (secondary edges are only sampled until the first rough bounce, src/edge.cpp:1396-1401)
 // and which strategy its boundary sample takes: the first number of its edge-sampler point < 0.5 -> GATHER, else HIERARCHY
 // (the reference's own per-sample coin, src/edge.cpp:1461-1472); one bit per depth in `vmask`.
-// A sample whose pixel's adjoint is exactly zero adds nothing: it is not traced (it still reaches the phase barriers) and gets
-// nrec = -1, which keeps it out of every work list, so the boundary stage and the sweep never see it.
+// The bands hold the samples of live pixels only (KernelArgs::live_pixels): a sample whose pixel's adjoint is exactly zero adds
+// nothing and never reaches this kernel.
 __global__ void __launch_bounds__(RB_BLOCK_TRACE, RB_MIN_BLOCKS_TRACE) k_bwd_trace(const __grid_constant__ DevScene sc, const __grid_constant__ KernelArgs ka) {
     const RenderParams& rp = ka.rp;
     RB_BLOCK_LOOP(t, ka.band_n) {
         bool act = t < ka.band_n;
-        SampleId id = band_sample(rp, ka.band_i0 + (act ? t : 0));
+        SampleId id = band_sample(ka, ka.band_i0 + (act ? t : 0));
         VertexRec* recs = ka.records + (size_t)(act ? t : 0) * ka.rec_per_sample;
-        const bool traced = act && !(ka.zero_cull && pixel_adjoint_is_zero(ka, id.pixel));
-        int n = bwd_trace(sc, rp, id.pixel, id.px, id.py, id.s, recs, 1, traced); // (-1 when not traced)
+        int n = bwd_trace(sc, rp, id.pixel, id.px, id.py, id.s, recs, 1, act); // (-1 when not traced)
         if (!act) continue;
         ka.nrec[t] = n;
         if (ka.dpos != nullptr) {
@@ -327,7 +326,6 @@ RB_D int sec_entry(const KernelArgs& ka, const SecRange& r, long long t) {
 // Stage 2a: edge pick of every listed path vertex (secondary edge sampling).  Writes the pick, its vertex and its edge per
 // slot and counts the picks per edge (aggregated per warp) for the counting sort below.
 __global__ void __launch_bounds__(RB_BLOCK_SEC, RB_MIN_BLOCKS_SEC) k_bwd_sec_pick(const __grid_constant__ DevScene sc, const __grid_constant__ KernelArgs ka) {
-    const RenderParams& rp = ka.rp;
     const SecRange r = sec_range(ka);
     const long long n = r.total;
     RB_BLOCK_LOOP(t, n) {
@@ -337,7 +335,7 @@ __global__ void __launch_bounds__(RB_BLOCK_SEC, RB_MIN_BLOCKS_SEC) k_bwd_sec_pic
             unsigned key = 0xffffffffu;
             if (e >= 0) {
                 int ts = e / ka.rec_per_sample, d = e - ts * ka.rec_per_sample;
-                SampleId id = band_sample(rp, ka.band_i0 + ts);
+                SampleId id = band_sample(ka, ka.band_i0 + ts);
                 VertexRec cur = ka.records[e];
                 EdgePick pk;
                 if (bwd_secondary_pick(sc, ka, id.pixel, id.s, d, cur, pk)) {
@@ -409,7 +407,6 @@ __global__ void __launch_bounds__(256) k_sec_scatter(const __grid_constant__ Ker
 #endif
 // Stage 2d: the two edge rays and their sub-paths, in edge order (neighbouring lanes aim at the same edge).
 __global__ void __launch_bounds__(RB_BLOCK_SEC, RB_MIN_BLOCKS_SEC) k_bwd_sec_shade(const __grid_constant__ DevScene sc, const __grid_constant__ KernelArgs ka) {
-    const RenderParams& rp = ka.rp;
     const long long n = ka.counters->n_picked;
     RB_BLOCK_LOOP(j, n) {
         RB_PHASE_SYNC();
@@ -417,7 +414,7 @@ __global__ void __launch_bounds__(RB_BLOCK_SEC, RB_MIN_BLOCKS_SEC) k_bwd_sec_sha
             unsigned t = ka.sec_order[j];
             int e = (int)ka.sec_vals[t];
             int ts = e / ka.rec_per_sample, d = e - ts * ka.rec_per_sample;
-            SampleId id = band_sample(rp, ka.band_i0 + ts);
+            SampleId id = band_sample(ka, ka.band_i0 + ts);
             VertexRec cur = ka.records[e];
             EdgePick pk = ka.picks[t];
             ka.dpos[e] = bwd_secondary_shade(sc, ka, id.pixel, id.s, d, cur, pk);
@@ -439,12 +436,11 @@ __global__ void __launch_bounds__(RB_BLOCK_SWEEP, RB_MIN_BLOCKS_SWEEP) k_bwd_swe
     cam_acc.base = cam_smem + threadIdx.x;
     cam_acc.stride = blockDim.x;
 #endif
-    const RenderParams& rp = ka.rp;
     const long long n = ka.counters->n_paths;
     RB_BLOCK_LOOP(t, n) {
         bool act = t < n;
         int ts = act ? ka.path_list[t] : 0;
-        SampleId id = band_sample(rp, ka.band_i0 + ts);
+        SampleId id = band_sample(ka, ka.band_i0 + ts);
         size_t base = (size_t)ts * ka.rec_per_sample;
         bwd_sweep(sc, ka, id.pixel, id.px, id.py, id.s, ka.records + base, 1, act ? ka.nrec[ts] : 0, ka.dpos ? ka.dpos + base : nullptr, cam_acc, act);
     }

@@ -34,8 +34,9 @@ struct KernelArgs {
     const float* d_image;
     float* screen_grad;
     DevDScene ds;
-    // ---- backward band state (rb_kernels.cu): the adjoint pass walks the image in bands of `band_n` pixel samples
-    long long band_i0;           // first dense sample index (owned pixel index * spp + s) of the band
+    // ---- backward band state (rb_kernels.cu): the adjoint pass walks the samples of the live pixels in bands of `band_n`
+    const int* live_pixels;      // viewport pixels of the owned rows whose adjoint is not zero (all of them without zero_cull), ascending
+    long long band_i0;           // first dense live sample index (index into live_pixels * spp + s) of the band
     int band_n;                  // samples in the band
     int rec_per_sample;          // max_bounces + 1 records per sample
     VertexRec* records;          // [band_n][rec_per_sample]
@@ -576,7 +577,7 @@ RB_D void bwd_sweep(const DevScene& sc, const KernelArgs& ka, int pixel, int px,
 // The three stages back to back for ONE sample: used by the host-compiled debug emulator (tools/cpu_emu) only.
 RB_D int backward_sample(const DevScene& sc, const KernelArgs& ka, int pixel, int px, int py, int s, VertexRec* recs, CamAcc& cam_acc) {
     const RenderParams& rp = ka.rp;
-    if (ka.zero_cull && pixel_adjoint_is_zero(ka, pixel)) return -1; // (like k_bwd_trace: the sample is not traced)
+    if (ka.zero_cull && pixel_adjoint_is_zero(ka, pixel)) return -1; // (like the bands, which hold the samples of live pixels only)
     int nrec = bwd_trace(sc, rp, pixel, px, py, s, recs, 1);
     if (nrec < 0) return -1;
     V3 dpos[RB_MAX_BOUNDARY_BOUNCES]; // (setup_backward rejects deeper paths when the stage runs)

@@ -827,6 +827,12 @@ extern "C" int rb_scene_last_backward_stats(const rb_scene* sc, float* bwd_ms3) 
     for (int i = 0; i < 3; i++) bwd_ms3[i] = sc->last_bwd_ms[i];
     return 0;
 }
+extern "C" int rb_scene_last_live_samples(const rb_scene* sc, long long* live_samples, long long* num_bands) {
+    if (!sc) return 1;
+    if (live_samples) *live_samples = sc->last_live_samples;
+    if (num_bands) *num_bands = sc->last_bands;
+    return 0;
+}
 extern "C" int rb_scene_last_exact_bytes(const rb_scene* sc, size_t* bytes) {
     if (!sc || !bytes) return 1;
     *bytes = sc->last_exact_bytes;

@@ -434,6 +434,13 @@ class Scene:  # src/redner.cpp:62-73, src/scene.cpp:63-307
         self._lib.rb_scene_last_exact_bytes(self._handle, C.byref(n))
         return n.value
 
+    def last_live_samples(self):
+        """(live samples, bands) of the last backward pass on this scene (rb_scene_last_live_samples): the samples of the pixels whose
+        d_rendered_image is not zero, and the bands the backward pass ran over them."""
+        n, b = C.c_longlong(0), C.c_longlong(0)
+        self._lib.rb_scene_last_live_samples(self._handle, C.byref(n), C.byref(b))
+        return n.value, b.value
+
     def last_stage_stats(self):
         """({kernel name: ms}, path_vertices, primary_hits) of the last render on this scene."""
         ms = (C.c_float * 4)()
