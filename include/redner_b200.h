@@ -112,6 +112,16 @@ typedef struct rb_area_light {
     int shape_id;
     float intensity[3];
     int two_sided, directly_visible;
+    /* Emission texture (no reference counterpart; DESIGN.md "Emission textures").  num_levels == 0 (the zero-initialised field) is no
+     * texture: the light emits `intensity` everywhere, as in the reference.  Otherwise the light emits intensity * E(uv) at a point of its
+     * shape, where E is this 1- or 3-channel mip-mapped texture (1 channel is broadcast to RGB) and uv the shape's texture coordinate there
+     * (its uvs, or the default per-triangle uvs, times uv_scale).  Rays from the camera and edge rays look it up with the footprint of the
+     * material textures at that hit; light samples and BSDF-sampled hits with a zero footprint.  Light selection and the point on the
+     * light are sampled as without a texture.  rb_scene_create and rb_scene_update refuse, with a message naming the emission texture, a
+     * channel count other than 1 or 3, num_levels outside [0, RB_MAX_MIP_LEVELS], a level without texels, a non-constant level without a
+     * positive size and a missing uv_scale.  rb_scene_update may add, change or remove the texture: it is a value of the light, like
+     * intensity. */
+    rb_texture emission;
 } rb_area_light;
 
 /* EnvironmentMap -- src/envmap.h:19-51, constructor src/redner.cpp:169-178.  `values` is the [h, w, 3] mip pyramid, the two
@@ -207,6 +217,12 @@ typedef struct rb_dscene_desc {
     int num_lights;
     float* const* light_intensity; /* host array of device pointers (3 floats each) -- src/area_light.h:38-43 */
     const rb_denvmap* envmap;      /* host pointer or NULL */
+    /* Gradients of the lights' emission textures (rb_area_light::emission): a host array of num_lights gradient pyramids (device memory),
+     * or NULL for none.  An entry with num_levels == 0 wants no gradient; then neither the texels and uv_scale nor the uvs and vertex
+     * positions receive what flows through that light's texture.  Otherwise the entry has the levels, sizes and channels of the scene's
+     * texture (rb_render refuses anything else, naming the emission texture), and uv_scale (2 floats) may be NULL.  The intensity gradient
+     * of a textured light is sum(d_Le * E(uv)). */
+    const rb_texture* light_emission;
 } rb_dscene_desc;
 
 typedef struct rb_scene rb_scene;
@@ -304,7 +320,8 @@ int rb_scene_last_exact_bytes(const rb_scene* scene, size_t* bytes);
  * A record is 13 signed 64-bit words: 10 limbs of a fixed-point number (limb k weighs 2^(32 k - 149)) and three counts of non-finite
  * contributions (+inf, -inf, NaN).  There are `count` records: one per camera gradient scalar, then one per float of every gradient
  * buffer of d_scene and screen_gradient_image, in the order: shapes (vertices, uvs, normals, colors), materials (the five textures:
- * levels, then uv_scale), light intensities, the environment map (levels, uv_scale, world_to_env), the screen-gradient image.  The
+ * levels, then uv_scale), light intensities, the lights' emission textures (for every light with one, when d_scene->light_emission is
+ * not NULL: levels, then uv_scale), the environment map (levels, uv_scale, world_to_env), the screen-gradient image.  The
  * position of a record depends on the structure of the descriptor only, never on where its buffers are; descriptors whose gradient
  * buffers overlap are refused.  `fingerprint` hashes that structure: compare it across ranks before summing.  Records live in memory
  * of the scene's device; `stream` as for rb_render, and both calls synchronise it. */
@@ -345,7 +362,9 @@ enum rb_scene_table_id {
     RB_TABLE_AREA_CDF_POOL,      /* double per emissive triangle: every light's triangle-area CDF */
     RB_TABLE_AREA_CDF_OFFSETS,   /* int per area light: first entry in the pool */
     RB_TABLE_PRIMARY_EDGE_PMF,   /* double per edge (src/edge.cpp:298-331); empty without primary-edge sampling */
-    RB_TABLE_PRIMARY_EDGE_CDF
+    RB_TABLE_PRIMARY_EDGE_CDF,
+    RB_TABLE_LIGHTS              /* the area lights as the kernels read them: { shape_id, intensity, two_sided, directly_visible } per light
+                                    (24 bytes), then from the next 16-byte boundary the lights' emission textures (rb_texture each) */
 };
 int rb_scene_table(const rb_scene* scene, int which, void* out, size_t bytes, size_t* size);
 

@@ -18,7 +18,7 @@ c_int_p = C.POINTER(C.c_int)
 
 # enum rb_scene_table_id
 RB_TABLES = ("bvh_nodes", "bvh_triangles", "light_pmf", "light_cdf", "light_areas", "area_cdf_pool", "area_cdf_offsets", "primary_edge_pmf",
-             "primary_edge_cdf")
+             "primary_edge_cdf", "lights")
 # enum rb_trace_flags
 RB_TRACE_ANY_HIT, RB_TRACE_BRUTE_FORCE = 1, 2
 # int64 words per record of rb_render_exact / rb_exact_round: 10 limbs, then the counts of +inf, -inf and NaN contributions
@@ -67,7 +67,7 @@ class rb_material(C.Structure):
 
 
 class rb_area_light(C.Structure):
-    _fields_ = [("shape_id", C.c_int), ("intensity", C.c_float * 3), ("two_sided", C.c_int), ("directly_visible", C.c_int)]
+    _fields_ = [("shape_id", C.c_int), ("intensity", C.c_float * 3), ("two_sided", C.c_int), ("directly_visible", C.c_int), ("emission", rb_texture)]
 
 
 class rb_envmap(C.Structure):
@@ -128,6 +128,7 @@ class rb_dscene_desc(C.Structure):
         ("num_materials", C.c_int), ("materials", C.POINTER(rb_material)),
         ("num_lights", C.c_int), ("light_intensity", C.POINTER(C.c_void_p)),
         ("envmap", C.POINTER(rb_denvmap)),
+        ("light_emission", C.POINTER(rb_texture)),
     ]
 
 

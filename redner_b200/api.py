@@ -172,9 +172,17 @@ class Shape:
 
 
 class AreaLight:
-    def __init__(self, shape_id: int, intensity: torch.Tensor, two_sided: bool = False, directly_visible: bool = True):
+    """`emission` (redner_b200 extension): None, or the light's emission texture, a Texture or an [h, w, 1 | 3] (or [1 | 3] constant) float32
+    tensor that may require grad.  The light then emits intensity * E(uv) at a point of its shape whose texture coordinate is uv
+    (DESIGN.md "Emission textures")."""
+
+    def __init__(self, shape_id: int, intensity: torch.Tensor, two_sided: bool = False, directly_visible: bool = True, emission=None):
         assert intensity.dtype == torch.float32 and tuple(intensity.shape) == (3,)
         self.shape_id, self.intensity, self.two_sided, self.directly_visible = shape_id, intensity, two_sided, directly_visible
+        self.emission = _as_texture(emission)
+        if self.emission is not None:
+            t = self.emission.texels
+            assert t.dtype == torch.float32 and t.shape[-1] in (1, 3) and t.dim() in (1, 3), "an emission texture has 1 or 3 channels"
 
 
 class EnvironmentMap:
@@ -229,7 +237,7 @@ _MaterialArgs = namedtuple("_MaterialArgs", "textures compute_specular_lighting 
 _LightArgs = namedtuple("_LightArgs", "shape_id intensity two_sided directly_visible")
 _EnvmapArgs = namedtuple("_EnvmapArgs", "values env_to_world world_to_env sample_cdf_ys sample_cdf_xs pdf_norm directly_visible")
 _OptionArgs = namedtuple("_OptionArgs", "num_samples max_bounces channels sampler_type use_primary_edge_sampling use_secondary_edge_sampling "
-                                        "sample_pixel_center pixel_filter device backend specular_models lens_radius focus_distance")
+                                        "sample_pixel_center pixel_filter device backend specular_models lens_radius focus_distance light_emission")
 
 
 def _ptr(backend, t, kind="float"):
@@ -377,6 +385,17 @@ class RenderFunction(torch.autograd.Function):
         args.append(models if any(models) else None)
         # the thin lens: lens_radius and focus_distance, None for a pinhole (the last group, so that no other entry moves)
         args += [t.cpu().contiguous() if t is not None else None for t in lens]
+        # the lights' emission textures: None when no light has one, else every light's number of mip levels (0: none), followed by the
+        # mips and uv_scale of each textured light (the last group, so that no other entry moves)
+        emission = [getattr(light, "emission", None) for light in scene.area_lights]
+        if any(t is not None for t in emission):
+            args.append(tuple(len(t.mipmap) if t is not None else 0 for t in emission))
+            for t in emission:
+                if t is not None:
+                    _serialize_texture(t, args, device)
+                    args.pop(-2 - len(t.mipmap))  # (the level count is in the tuple)
+        else:
+            args.append(None)
         return args
 
     @staticmethod
@@ -384,7 +403,8 @@ class RenderFunction(torch.autograd.Function):
         """serialize_scene's argument list, read in one pass.  Besides serialize_scene, this is the only code that knows the list's layout.
 
         Returns a namespace of `camera_args`, `shape_args`, `mat_args`, `light_args` (lists), `env_args` (None without an environment map)
-        and `option_args`: the entries serialize_scene wrote for each, as the named tuples above.  A material's `textures` are five
+        and `option_args`: the entries serialize_scene wrote for each, as the named tuples above; `emission_args` holds each light's emission
+        texture (a _TextureArgs, or None).  A material's `textures` are five
         _TextureArgs or None (diffuse, specular, roughness, generic, normal map); the environment map's `values` is one.  `pos` holds the
         same structure with the position in `args` of each entry in place of the entry.  `args` is the list itself."""
         k = 3  # (after the numbers of shapes, materials and lights)
@@ -425,6 +445,15 @@ class RenderFunction(torch.autograd.Function):
             rest, rest_pos = entries(len(_EnvmapArgs._fields) - 1)
             a.env_args, a.pos.env_args = _EnvmapArgs(values, *rest), _EnvmapArgs(positions, *rest_pos)
         a.option_args, a.pos.option_args = take(_OptionArgs)
+        levels = a.option_args.light_emission or (0,) * args[2]
+        a.emission_args, a.pos.emission_args = [], []
+        for n in levels:
+            t, q = None, None
+            if n:
+                (mips, mip_pos), (uv, uv_pos) = entries(n), entries(1)
+                t, q = _TextureArgs(list(mips), uv[0]), _TextureArgs(list(mip_pos), uv_pos[0])
+            a.emission_args.append(t)
+            a.pos.emission_args.append(q)
         assert k == len(args), "serialize_scene's list has %d entries, its layout %d" % (len(args), k)
         return a
 
@@ -458,7 +487,9 @@ class RenderFunction(torch.autograd.Function):
             # (the keyword only for a non-default lobe: a backend without one renders Blinn-Phong)
             materials.append(rb.Material(*textures, m.compute_specular_lighting, m.two_sided, m.use_vertex_color,
                                          **({} if models is None or not models[i] else {"specular_model": models[i]})))
-        lights = [rb.AreaLight(l.shape_id, fp(l.intensity), l.two_sided, l.directly_visible) for l in c.light_args]
+        # (the keyword only for a textured light: a backend without emission textures renders the others)
+        lights = [rb.AreaLight(l.shape_id, fp(l.intensity), l.two_sided, l.directly_visible,
+                               **({} if e is None else {"emission": _native_texture(rb, rb.TextureN, 0, e)})) for l, e in zip(c.light_args, c.emission_args)]
         envmap = None
         if c.env_args is not None:
             e = c.env_args
@@ -499,7 +530,8 @@ class RenderFunction(torch.autograd.Function):
         The buffers, in the order they are allocated: `camera` (the eight of rb.DCamera, None where there is none), `lens` (None for a
         pinhole, else the two floats d(lens_radius), d(focus_distance) in one buffer, whose halves are the grads of the two entries), `shapes` ((vertices,
         uvs, normals, colors) per shape), `materials` (per material its five textures, each None or (mips, uv_scale)), `intensities` (per
-        light) and `envmap` (None or (mips, uv_scale, world_to_env)).  `grads` maps the position in serialize_scene's list of each argument
+        light), `envmap` (None or (mips, uv_scale, world_to_env)) and `emission` (per light None or the (mips, uv_scale) of its emission
+        texture).  `grads` maps the position in serialize_scene's list of each argument
         that has a buffer to that buffer."""
         rb, dev, p = c.option_args.backend, c.option_args.device, c.pos
         z = zeros or (lambda *shape: torch.zeros(*shape, device=dev))
@@ -536,10 +568,12 @@ class RenderFunction(torch.autograd.Function):
             values = c.env_args.values
             g.envmap = texture(values, p.env_args.values) + (buf(p.env_args.world_to_env, 4, 4),)
             d_envmap = rb.DEnvironmentMap(_native_texture(rb, rb.Texture3, 3, values, g.envmap[:2]), fp(g.envmap[2]))
+        g.emission = [texture(t, q) for t, q in zip(c.emission_args, p.emission_args)]
         d_materials = [rb.DMaterial(*[_native_texture(rb, cls, nch, t, b) for (cls, nch), t, b in zip(_material_textures(rb), m.textures, bufs)])
                        for m, bufs in zip(c.mat_args, g.materials)]
         g.d_scene = rb.DScene(rb.DCamera(*[fp(t) for t in g.camera], **({} if g.lens is None else {"lens": fp(g.lens)})), [rb.DShape(*[fp(t) for t in b]) for b in g.shapes], d_materials,
-                              [rb.DAreaLight(fp(t)) for t in g.intensities], d_envmap, dev.type == "cuda", dev.index if dev.index is not None else -1)
+                              [rb.DAreaLight(fp(t), **({} if b is None else {"emission": _native_texture(rb, rb.TextureN, 0, e, b)}))
+                               for t, e, b in zip(g.intensities, c.emission_args, g.emission)], d_envmap, dev.type == "cuda", dev.index if dev.index is not None else -1)
         return g
 
     @staticmethod

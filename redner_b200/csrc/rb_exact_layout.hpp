@@ -9,6 +9,7 @@
 // buffers.  Records (rb_exact.cuh), the form in which accumulators are summed across calls and devices, are numbered by the structure
 // of the descriptor alone: the camera scalars, then one record per float of every gradient buffer in the order exact_layout visits
 // them -- shapes (vertices, uvs, normals, colours), materials (the five textures: their levels, then uv_scale), light intensities, the
+// lights' emission textures (only with d_scene.light_emission, and only for the lights with a texture: levels, then uv_scale), the
 // environment map (levels, uv_scale), world_to_env, the screen-gradient image.  Overlapping buffers have no such position: the entry
 // points that take or give records (rb_exact_record_count, rb_render_exact, rb_exact_round) refuse descriptors whose gradient buffers
 // overlap.  ExactLayout::fingerprint hashes that structure, so that callers can check that their records line up before they sum them.
@@ -42,6 +43,7 @@ struct ExactLayout {
     std::vector<rb_dshape> shapes;      // the descriptors with virtual addresses
     std::vector<rb_material> materials;
     std::vector<float*> lights;
+    std::vector<rb_texture> light_emission; // (empty without d_scene.light_emission)
     rb_texture env_values;
     float* env_w2e = nullptr;
     float* screen_grad = nullptr;
@@ -49,9 +51,9 @@ struct ExactLayout {
 
 // Floats of every gradient buffer the backward pass of `sc` can write through `ka.ds` / `ka.screen_grad` (as set up by
 // setup_backward), with shape and texture sizes from the scene's descriptors (`shapes`, `materials`): the kernels index gradient
-// buffers like the scene's own buffers.
-inline void exact_layout(const rb_dscene_desc& d, const rb_shape* shapes, const rb_material* materials, const DevScene& sc, const KernelArgs& ka,
-                         ExactLayout& out) {
+// buffers like the scene's own buffers.  `emission`: the lights' emission textures (host copies).
+inline void exact_layout(const rb_dscene_desc& d, const rb_shape* shapes, const rb_material* materials, const rb_texture* emission, const DevScene& sc,
+                         const KernelArgs& ka, ExactLayout& out) {
     struct Span {
         uintptr_t begin, end;
         long long rec; // record of its first float
@@ -95,6 +97,10 @@ inline void exact_layout(const rb_dscene_desc& d, const rb_shape* shapes, const 
         add_texture(mt.normal_map, dm.normal_map, 3);
     }
     for (int l = 0; l < d.num_lights; l++) add(d.light_intensity[l], 3);
+    // (a descriptor without emission gradients, or with none for a light without a texture, visits nothing here)
+    if (d.light_emission != nullptr)
+        for (int l = 0; l < d.num_lights; l++)
+            if (emission[l].num_levels > 0) add_texture(emission[l], d.light_emission[l], std::max(emission[l].channels, 1));
     if (sc.has_envmap) add_texture(sc.env.values, ka.ds.env_values, 3);
     add(ka.ds.env_w2e, 16);
     add(ka.screen_grad, 2LL * ka.rp.vp_w * ka.rp.vp_h);
@@ -161,23 +167,26 @@ inline void exact_layout(const rb_dscene_desc& d, const rb_shape* shapes, const 
     }
     out.lights.assign(d.light_intensity, d.light_intensity + d.num_lights);
     for (float*& l : out.lights) l = virt(l);
+    out.light_emission.clear();
+    if (d.light_emission != nullptr)
+        for (int l = 0; l < d.num_lights; l++) out.light_emission.push_back(virt_texture(d.light_emission[l]));
     out.env_values = virt_texture(ka.ds.env_values);
     out.env_w2e = virt(ka.ds.env_w2e);
     out.screen_grad = virt(ka.screen_grad);
 }
 
 // The records of a backward pass of `opt` over d_scene / screen_grad on a scene (camera `cam`, generic-texture width `max_generic`,
-// descriptors `shapes` / `materials`, device-side scene `sc`): the checks and the layout of rb_render's backward pass, and the refusal of
+// descriptors `shapes` / `materials`, the lights' emission textures `emission`, device-side scene `sc`): the checks and the layout of rb_render's backward pass, and the refusal of
 // overlapping gradient buffers.  `who` prefixes the messages of this function's own checks.  Returns the error message, or null.
 inline const char* exact_record_layout(const char* who, const rb_options& opt, const rb_camera& cam, int max_generic, const rb_dscene_desc* d_scene,
-                                       float* screen_grad, const rb_shape* shapes, const rb_material* materials, const DevScene& sc, KernelArgs& ka,
-                                       ExactLayout& xl, std::string& err) {
+                                       float* screen_grad, const rb_shape* shapes, const rb_material* materials, const rb_texture* emission,
+                                       const DevScene& sc, KernelArgs& ka, ExactLayout& xl, std::string& err) {
     if (d_scene == nullptr) return (err = std::string(who) + ": null d_scene").c_str();
     static const float no_image = 0.f; // (the layout does not depend on the image: any non-null d_image passes the checks)
     const char* e = setup_kernel_args(opt, cam, max_generic, 0, 1, 1, nullptr, &no_image, d_scene, screen_grad, ka);
-    if (e == nullptr) e = setup_backward(*d_scene, sc, ka);
+    if (e == nullptr) e = setup_backward(*d_scene, sc, emission, ka);
     if (e != nullptr) return e;
-    exact_layout(*d_scene, shapes, materials, sc, ka, xl);
+    exact_layout(*d_scene, shapes, materials, emission, sc, ka, xl);
     if (xl.overlaps) return (err = std::string(who) + ": gradient buffers of d_scene overlap; records need disjoint buffers").c_str();
     return nullptr;
 }

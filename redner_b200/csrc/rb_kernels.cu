@@ -147,11 +147,13 @@ static int render_pass(const rb_scene* scene_, const rb_options* opt, float* ima
     // The feature-free instantiation of the kernels (rb_kernels_lean.cu) serves the common configuration, and its diffuse-only refinement
     // (rb_kernels_diffuse.cu) the scenes of that configuration whose materials are all diffuse; `kern` holds the kernels of the chosen
     // instantiation, and every launch of one of them below goes through it.  The materials are read from the scene's host copies on every
-    // call: rb_scene_update may have changed their flags.  Neither set has the GGX lobe (RB_GGX is false there).
+    // call: rb_scene_update may have changed their flags.  Neither set has the GGX lobe (RB_GGX is false there), nor emission textures
+    // (RB_LIGHT_TEX), which the lights' host copies tell likewise.
     const bool lean_allowed = getenv("RB_NO_LEAN") == nullptr;       // (test hook: force the general kernels)
     const bool diffuse_allowed = getenv("RB_NO_DIFFUSE") == nullptr; // (test hook: force the lean kernels where the diffuse ones would run)
     const DevCamera& cam = scene->dev.cam;
-    const bool lean = lean_allowed && !materials_use_ggx(scene->materials.data(), (int)scene->materials.size()) && rp.only_radiance && !scene->dev.has_envmap && cam.type == RB_CAMERA_PERSPECTIVE && !cam.has_distortion &&
+    const bool lean = lean_allowed && !materials_use_ggx(scene->materials.data(), (int)scene->materials.size()) && !lights_use_emission(scene->light_emission) &&
+                      rp.only_radiance && !scene->dev.has_envmap && cam.type == RB_CAMERA_PERSPECTIVE && !cam.has_distortion &&
                       cam.filter_type == RB_FILTER_BOX && cam.filter_width == 1.0f && cam.lens_radius == 0;
     const bool diffuse = lean && diffuse_allowed && materials_diffuse_only(scene->materials.data(), (int)scene->materials.size());
     const RenderKernels kern = diffuse ? rb_diffuse::render_kernels() : lean ? rb_lean::render_kernels() : render_kernels();
@@ -198,13 +200,13 @@ static int render_pass(const rb_scene* scene_, const rb_options* opt, float* ima
         for (int i = EV_AFTER_BANDS; i <= EV_END; i++) RB_CUDA_OK(cudaEventRecord(ev[i], stream));
     }
     if (d_image != nullptr) {
-        if (const char* err = setup_backward(*d_scene, scene->dev, ka)) {
+        if (const char* err = setup_backward(*d_scene, scene->dev, scene->light_emission.data(), ka)) {
             rb_set_error(err);
             return 1;
         }
         ExactLayout xl;
         if (det) {
-            exact_layout(*d_scene, scene->shapes.data(), scene->materials.data(), scene->dev, ka, xl);
+            exact_layout(*d_scene, scene->shapes.data(), scene->materials.data(), scene->light_emission.data(), scene->dev, ka, xl);
             if (xo && xl.overlaps) {
                 rb_set_error("rb_render_exact: gradient buffers of d_scene overlap; records need disjoint buffers");
                 return 1;
@@ -286,7 +288,8 @@ static int render_pass(const rb_scene* scene_, const rb_options* opt, float* ima
             const size_t n_edges = (size_t)std::max(scene->dev.num_edges, 1), n_rec = (size_t)band * ka.rec_per_sample;
             d_shapes = (rb_dshape*)take(std::max(1, d_scene->num_shapes) * sizeof(rb_dshape));
             d_mats = (rb_material*)take(std::max(1, d_scene->num_materials) * sizeof(rb_material));
-            d_lights = (float**)take(std::max(1, d_scene->num_lights) * sizeof(float*));
+            // (the intensity-gradient pointers, then the gradients of the emission textures: light_d_emission, rb_types.cuh)
+            d_lights = (float**)take(std::max<size_t>(light_table_offset(d_scene->num_lights * sizeof(float*)) + d_scene->num_lights * sizeof(rb_texture), 8));
             exact_acc = (long long*)take(det ? (size_t)(xl.num_acc + 1) * RB_EXACT_WORDS * sizeof(long long) : 0);
             exact_ranges = (ExactRange*)take(det ? std::max<size_t>(xl.ranges.size(), 1) * sizeof(ExactRange) : 0);
             exact_rec_first = (long long*)take(xo ? std::max<size_t>(xl.rec_first.size(), 1) * sizeof(long long) : 0);
@@ -337,12 +340,14 @@ static int render_pass(const rb_scene* scene_, const rb_options* opt, float* ima
         // (deterministic mode: the descriptors with the virtual addresses of the accumulators; no kernel reads a gradient buffer)
         const rb_dshape* h_shapes = det ? xl.shapes.data() : d_scene->shapes;
         const rb_material* h_mats = det ? xl.materials.data() : d_scene->materials;
-        float* const* h_lights = det ? xl.lights.data() : d_scene->light_intensity;
+        const std::vector<unsigned long long> h_lights = light_table_words(det ? xl.lights.data() : d_scene->light_intensity,
+                                                                           det ? (xl.light_emission.empty() ? nullptr : xl.light_emission.data()) : d_scene->light_emission,
+                                                                           d_scene->num_lights);
         if (d_scene->num_shapes) RB_CUDA_OK(cudaMemcpyAsync(d_shapes, h_shapes, d_scene->num_shapes * sizeof(rb_dshape), cudaMemcpyHostToDevice, stream));
         if (d_scene->num_materials)
             RB_CUDA_OK(cudaMemcpyAsync(d_mats, h_mats, d_scene->num_materials * sizeof(rb_material), cudaMemcpyHostToDevice, stream));
         if (d_scene->num_lights)
-            RB_CUDA_OK(cudaMemcpyAsync(d_lights, h_lights, d_scene->num_lights * sizeof(float*), cudaMemcpyHostToDevice, stream));
+            RB_CUDA_OK(cudaMemcpyAsync(d_lights, h_lights.data(), h_lights.size() * 8, cudaMemcpyHostToDevice, stream));
         if (det) {
             if (!xl.ranges.empty())
                 RB_CUDA_OK(cudaMemcpyAsync(exact_ranges, xl.ranges.data(), xl.ranges.size() * sizeof(ExactRange), cudaMemcpyHostToDevice, stream));
@@ -509,7 +514,7 @@ extern "C" int rb_exact_record_count(const rb_scene* scene, const rb_options* op
     ExactLayout xl;
     std::string err;
     if (const char* e = exact_record_layout("rb_exact_record_count", *opt, scene->cam, scene->max_generic_texture_dimension, d_scene, screen_grad,
-                                            scene->shapes.data(), scene->materials.data(), scene->dev, ka, xl, err)) {
+                                            scene->shapes.data(), scene->materials.data(), scene->light_emission.data(), scene->dev, ka, xl, err)) {
         rb_set_error(e);
         return 1;
     }
@@ -542,7 +547,7 @@ extern "C" int rb_exact_round(const rb_scene* scene, const rb_options* opt, cons
     ExactLayout xl;
     std::string err;
     if (const char* e = exact_record_layout("rb_exact_round", *opt, scene->cam, scene->max_generic_texture_dimension, d_scene, screen_grad, scene->shapes.data(),
-                                            scene->materials.data(), scene->dev, ka, xl, err)) {
+                                            scene->materials.data(), scene->light_emission.data(), scene->dev, ka, xl, err)) {
         rb_set_error(e);
         return 1;
     }

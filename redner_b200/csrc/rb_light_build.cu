@@ -107,10 +107,12 @@ int rb_build_lights(rb_scene* sc, bool geometry, cudaStream_t stream) {
     double *d_pmf, *d_cdf, *d_areas, *d_pool;
     int* d_off;
     LightAux* aux;
-    if (scene_table(sc, SS_LIGHTS, L, stream, &d_lights) || scene_table(sc, SS_LIGHT_PMF, sc->dev.num_lights, stream, &d_pmf) ||
+    unsigned long long* d_table; // the DevLights, then the lights' emission textures (sc->light_table, rb_types.cuh)
+    if (scene_table(sc, SS_LIGHTS, sc->light_table.size(), stream, &d_table) || scene_table(sc, SS_LIGHT_PMF, sc->dev.num_lights, stream, &d_pmf) ||
         scene_table(sc, SS_LIGHT_CDF, sc->dev.num_lights, stream, &d_cdf) || scene_table(sc, SS_LIGHT_AUX, 1, stream, &aux))
         return 1;
-    if (L > 0) RB_CUDA_OK(cudaMemcpyAsync(d_lights, sc->lights.data(), sizeof(DevLight) * L, cudaMemcpyHostToDevice, stream));
+    d_lights = (DevLight*)d_table;
+    if (L > 0) RB_CUDA_OK(cudaMemcpyAsync(d_table, sc->light_table.data(), sizeof(unsigned long long) * sc->light_table.size(), cudaMemcpyHostToDevice, stream));
     if (geometry) {
         std::vector<int>& off = sc->light_offsets;
         off.assign(L + 1, 0);

@@ -42,6 +42,8 @@ typedef float Real;
 #define RB_PIXEL_BOX(cam) true
 #define RB_GGX(m) false
 #define RB_CAM_LENS(cam) false
+#define RB_LIGHT_TEX(t) false
+#define RB_LIGHT_TEX_KERNELS 0
 #else
 #define RB_ENVMAP(sc) ((sc).has_envmap != 0)
 #define RB_CAM_GENERAL(cam) ((cam).type != RB_CAMERA_PERSPECTIVE || (cam).has_distortion != 0)
@@ -53,6 +55,10 @@ typedef float Real;
 #define RB_GGX(m) ((m).specular_model == RB_SPECULAR_GGX)
 // The thin lens (rb_camera::lens_radius) likewise: rb_render keeps lens cameras off the lean and diffuse-only sets.
 #define RB_CAM_LENS(cam) ((cam).lens_radius > 0)
+// The emission texture of an area light (rb_area_light::emission, `t`) likewise: rb_render keeps scenes with one off those sets.
+#define RB_LIGHT_TEX(t) ((t).num_levels > 0)
+// (for the adjoint's bookkeeping, which is compiled only where RB_LIGHT_TEX can be true, so that the lean kernels stay as they were)
+#define RB_LIGHT_TEX_KERNELS 1
 #endif
 // Material features.  rb_kernels_diffuse.cu compiles the lean kernels once more with RB_DIFFUSE defined as well: no material
 // computes specular lighting, uses vertex colours or has a normal map -- the diffuse-only scenes of shape and pose optimisation.

@@ -115,14 +115,49 @@ RB_D void sample_light(const DevScene& sc, D3 p_d, double light_sel, double tri_
     rec.unoccluded = !any_hit(sc, sh);
 }
 
-// Emission seen along a primary / edge ray (radiance channel of accumulate_primary_contribs).
+// Adjoint of light_sample_uv (rb_shape.cuh): d(uv) into the light's uv gradient buffer `d_uvs` (for a shape with uvs).
+RB_D void d_light_sample_uv(const rb_shape& s, int tri, V2 sample, V2 d_uv, float* d_uvs) {
+    TriAttribs a;
+    tri_attribs(s, tri, a);
+    Real r = sqrt(sample.x);
+    Real b1 = 1 - r, b2 = r * sample.y;
+    agg_add2(d_uvs + 2 * (size_t)a.uv_ind[0], d_uv * (1 - (b1 + b2)));
+    agg_add2(d_uvs + 2 * (size_t)a.uv_ind[1], d_uv * b1);
+    agg_add2(d_uvs + 2 * (size_t)a.uv_ind[2], d_uv * b2);
+}
+// Emission texture of area light `l` (RB_LIGHT_TEX) at texture coordinate uv with footprint (du_dxy, dv_dxy), broadcast to RGB from one
+// channel: the factor E(uv) of Le = intensity * E(uv).
+RB_D V3 light_tex_eval(const rb_texture& t, V2 uv, V2 du_dxy, V2 dv_dxy) { return tex_eval(t, t.channels, uv, du_dxy, dv_dxy); }
+// Adjoint of that lookup for d(loss)/d(E) `d_E`: scatters into the light's gradient texture, and returns d(uv) (d(du_dxy) and d(dv_dxy)
+// are added to the two references).  Nothing when the backward pass has no gradient texture for the light.
+RB_D V2 d_light_tex_eval(const DevScene& sc, const DevDScene& ds, int l, V2 uv, V2 du_dxy, V2 dv_dxy, V3 d_E, V2& d_du_dxy, V2& d_dv_dxy) {
+    const rb_texture& t = light_emission(sc, l);
+    const rb_texture& dt = light_d_emission(sc, ds, l);
+    if (dt.num_levels <= 0) return zero2();
+    const Real d0 = t.channels == 1 ? sum(d_E) : d_E.x; // (one channel is read three times)
+    if (tex_is_constant(t)) {
+        if (t.channels == 3) agg_add3(dt.texels[0], d_E);
+        else agg_add1(dt.texels[0], d0);
+        return zero2();
+    }
+    TexAdjoint r = d_tex_eval_mip(t, dt, t.channels, uv, du_dxy, dv_dxy, d0, d_E.y, d_E.z);
+    d_du_dxy += r.d_du_dxy;
+    d_dv_dxy += r.d_dv_dxy;
+    return r.d_uv;
+}
+
+// Emission seen along a primary / edge ray (radiance channel of accumulate_primary_contribs).  An emission texture is looked up with the
+// footprint the material textures use at the hit.
 RB_D V3 hit_emission(const DevScene& sc, const Isect& is, const SurfacePoint& sp, V3 wi) {
     if (!is.valid()) return zero3();
     const rb_shape& shape = sc.shapes[is.shape_id];
     if (shape.light_id >= 0) {
         const DevLight& light = sc.lights[shape.light_id];
-        if (light.directly_visible && (light.two_sided || dot(wi, sp.shading_frame.n) > 0))
+        if (light.directly_visible && (light.two_sided || dot(wi, sp.shading_frame.n) > 0)) {
+            const rb_texture& et = light_emission(sc, shape.light_id);
+            if (RB_LIGHT_TEX(et)) return mk3(light.intensity[0], light.intensity[1], light.intensity[2]) * light_tex_eval(et, sp.uv, sp.du_dxy, sp.dv_dxy);
             return mk3(light.intensity[0], light.intensity[1], light.intensity[2]);
+        }
     }
     return zero3();
 }
@@ -161,6 +196,9 @@ RB_D V3 vertex_estimate(const DevScene& sc, const rb_material& mat, const Surfac
                     G = fabs(dot(wo, lp.geom_normal)) / dist_sq;
                     pdf_nee = (Real)(sc.light_pmf[lshape.light_id] / sc.light_areas[lshape.light_id]);
                     Le = mk3(light.intensity[0], light.intensity[1], light.intensity[2]);
+                    // (an emission texture: at the sample's uv, unfiltered like the environment map's lookups)
+                    const rb_texture& et = light_emission(sc, lshape.light_id);
+                    if (RB_LIGHT_TEX(et)) Le = Le * light_tex_eval(et, light_sample_uv(lshape, ls.isect.tri_id, ls.uv), zero2(), zero2());
                     on = true;
                 }
             }
@@ -201,7 +239,10 @@ RB_D V3 vertex_estimate(const DevScene& sc, const rb_material& mat, const Surfac
                     if (light.two_sided || dot(-wo, bp.shading_frame.n) > 0) {
                         Real G = fabs(dot(wo, bp.geom_normal)) / dist_sq;
                         Real pdf_nee = (Real)(sc.light_pmf[bshape.light_id] * (1.0 / sc.light_areas[bshape.light_id])) / G;
-                        scatter = (mis_power2(pdf_nee, pdf_b) / pdf_b) * f * mk3(light.intensity[0], light.intensity[1], light.intensity[2]);
+                        V3 Le = mk3(light.intensity[0], light.intensity[1], light.intensity[2]);
+                        const rb_texture& et = light_emission(sc, bshape.light_id);
+                        if (RB_LIGHT_TEX(et)) Le = Le * light_tex_eval(et, bp.uv, zero2(), zero2());
+                        scatter = (mis_power2(pdf_nee, pdf_b) / pdf_b) * f * Le;
                     }
                 }
                 scatter_factor = f / pdf_b;
@@ -360,6 +401,11 @@ RB_D VertexAdjoint d_vertex(const DevScene& sc, const DevDScene& ds, const Verte
         V3 wo = zero3(), dir = zero3(), Le = zero3();
         Real dist_sq = 1, pdf_nee = 0;
         bool ok = false;
+#if RB_LIGHT_TEX_KERNELS
+        bool tex_l = false; // an emission texture (RB_LIGHT_TEX): its value E_l at the sample's uv `luv`
+        V3 E_l = zero3();
+        V2 luv = zero2();
+#endif
         if (area) {
             const rb_shape& lshape = sc.shapes[lis.shape_id];
             lp = sample_light_triangle(lshape, lis.tri_id, cur.light.uv);
@@ -370,6 +416,15 @@ RB_D VertexAdjoint d_vertex(const DevScene& sc, const DevDScene& ds, const Verte
                 const DevLight& light = sc.lights[lshape.light_id];
                 if (light.two_sided || dot(-wo, lp.shading_frame.n) > 0) {
                     Le = mk3(light.intensity[0], light.intensity[1], light.intensity[2]);
+#if RB_LIGHT_TEX_KERNELS
+                    const rb_texture& et = light_emission(sc, lshape.light_id);
+                    if (RB_LIGHT_TEX(et)) {
+                        tex_l = true;
+                        luv = light_sample_uv(lshape, lis.tri_id, cur.light.uv);
+                        E_l = light_tex_eval(et, luv, zero2(), zero2());
+                        Le = Le * E_l;
+                    }
+#endif
                     pdf_nee = (Real)(sc.light_pmf[lshape.light_id] * (1.0 / sc.light_areas[lshape.light_id]));
                     ok = true;
                 }
@@ -399,7 +454,22 @@ RB_D VertexAdjoint d_vertex(const DevScene& sc, const DevDScene& ds, const Verte
                 Real d_G = wgt * sum(d_nee * f * Le);
                 Real d_area = -d_pdf_nee * pdf_nee / shape_tri_area(lshape, lis.tri_id);
                 d_shape_tri_area(lshape, lis.tri_id, d_area, d_lv);
+#if RB_LIGHT_TEX_KERNELS
+                if (tex_l) { // Le = intensity * E(uv): into the intensity, the texture and the light's uvs
+                    const int lid = lshape.light_id;
+                    const DevLight& light = sc.lights[lid];
+                    const V3 d_Le = wgt * G * (d_nee * f);
+                    agg_add3(ds.light_intensity[lid], d_Le * E_l);
+                    V2 d_du = zero2(), d_dv = zero2();
+                    V2 d_uv = d_light_tex_eval(sc, ds, lid, luv, zero2(), zero2(), d_Le * mk3(light.intensity[0], light.intensity[1], light.intensity[2]), d_du, d_dv);
+                    const rb_dshape& dls = ds.shapes[lis.shape_id];
+                    if (lshape.uvs && dls.uvs) d_light_sample_uv(lshape, lis.tri_id, cur.light.uv, d_uv, dls.uvs);
+                } else {
+                    agg_add3(ds.light_intensity[lshape.light_id], wgt * G * (d_nee * f));
+                }
+#else
                 agg_add3(ds.light_intensity[lshape.light_id], wgt * G * (d_nee * f));
+#endif
                 d_cos_l = cos_l > 0 ? d_G / dist_sq : -d_G / dist_sq;
                 dir_l = dir;
                 dist_sq_l = dist_sq;
@@ -420,6 +490,10 @@ RB_D VertexAdjoint d_vertex(const DevScene& sc, const DevDScene& ds, const Verte
     }
     // ---- BSDF-sampled continuation (pre): the ray hit something (:339-518) or left the scene into the map (:520-590)
     SurfacePoint bp;
+#if RB_LIGHT_TEX_KERNELS
+    bool tex_b = false; // the hit is on a light with an emission texture (RB_LIGHT_TEX); d(uv) of the hit
+    V2 d_buv = zero2();
+#endif
     if (nxt != nullptr && (nxt->isect.valid() || RB_ENVMAP(sc))) {
         const bool hit = nxt->isect.valid();
         const Isect& bis = nxt->isect;
@@ -446,11 +520,32 @@ RB_D VertexAdjoint d_vertex(const DevScene& sc, const DevDScene& ds, const Verte
                     if (light.two_sided || dot(-wo, bp.shading_frame.n) > 0) {
                         Real G = fabs(dot(wo, bp.geom_normal)) / dist_sq;
                         V3 Le = mk3(light.intensity[0], light.intensity[1], light.intensity[2]);
+#if RB_LIGHT_TEX_KERNELS
+                        const rb_texture& et = light_emission(sc, bshape.light_id);
+                        V3 E_b = zero3();
+                        if (RB_LIGHT_TEX(et)) {
+                            tex_b = true;
+                            E_b = light_tex_eval(et, bp.uv, zero2(), zero2());
+                            Le = Le * E_b;
+                        }
+#endif
                         Real pdf_nee = (Real)(sc.light_pmf[bshape.light_id] * (1.0 / sc.light_areas[bshape.light_id])) / G;
                         Real wgt = mis_power2(pdf_nee, pdf_b) / pdf_b;
                         out.d_thr += d_contrib * (wgt * f * Le);
                         d_f += wgt * (d_scatter * Le);
+#if RB_LIGHT_TEX_KERNELS
+                        if (tex_b) { // into the intensity and the texture; d(uv) reaches the hit's uvs and vertices through d_make_surface_point
+                            const V3 d_Le = wgt * (d_scatter * f);
+                            agg_add3(ds.light_intensity[bshape.light_id], d_Le * E_b);
+                            V2 d_du = zero2(), d_dv = zero2();
+                            d_buv = d_light_tex_eval(sc, ds, bshape.light_id, bp.uv, zero2(), zero2(),
+                                                     d_Le * mk3(light.intensity[0], light.intensity[1], light.intensity[2]), d_du, d_dv);
+                        } else {
+                            agg_add3(ds.light_intensity[bshape.light_id], wgt * (d_scatter * f));
+                        }
+#else
                         agg_add3(ds.light_intensity[bshape.light_id], wgt * (d_scatter * f));
+#endif
                     }
                 }
                 dir_b = dir;
@@ -515,6 +610,9 @@ RB_D VertexAdjoint d_vertex(const DevScene& sc, const DevDScene& ds, const Verte
         d_dir += d_length_sq(dir_b, d_dist_sq);
         SurfacePoint d_bp = next.d_point;
         d_bp.position += d_dir;
+#if RB_LIGHT_TEX_KERNELS
+        if (tex_b) d_bp.uv += d_buv;
+#endif
         DRay d_ray = zero_dray();
         RayDiff d_rd_b = zero_raydiff();
         Ray bray;

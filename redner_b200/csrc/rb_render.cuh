@@ -152,11 +152,26 @@ RB_HD bool boundary_stage_runs(const DevScene& sc, const RenderParams& rp) {
 }
 // The primary-edge pass of the backward pass runs.
 RB_HD bool primary_edge_pass_runs(const DevScene& sc) { return sc.use_primary_edge && sc.num_edges > 0 && sc.prim_edge_cdf != nullptr; }
-// Checks the gradient descriptor against the scene and the options, and points the environment-map gradients of `ka.ds` at
-// d_scene's.  Returns the error message, or null.  Each driver fills the shape, material, light and camera gradients itself.
-inline const char* setup_backward(const rb_dscene_desc& d_scene, const DevScene& sc, KernelArgs& ka) {
+// The gradients of the lights' emission textures (rb_dscene_desc::light_emission) against the scene's textures (`emission`, host copies,
+// one per area light).  Returns the error message, or null.
+inline const char* check_light_emission_grads(const rb_dscene_desc& d_scene, const rb_texture* emission) {
+    if (d_scene.light_emission == nullptr) return nullptr;
+    for (int l = 0; l < d_scene.num_lights; l++) {
+        const rb_texture &dt = d_scene.light_emission[l], &t = emission[l];
+        if (dt.num_levels == 0) continue;
+        bool same = dt.num_levels == t.num_levels && dt.channels == t.channels;
+        for (int k = 0; same && k < t.num_levels; k++) same = dt.width[k] == t.width[k] && dt.height[k] == t.height[k] && dt.texels[k] != nullptr;
+        if (!same) return "rb_render: a light's emission texture gradient (d_scene light_emission) needs the levels, sizes and channels of the light's emission texture";
+    }
+    return nullptr;
+}
+// Checks the gradient descriptor against the scene (`emission`: its lights' emission textures, host copies) and the options, and points
+// the environment-map gradients of `ka.ds` at d_scene's.  Returns the error message, or null.  Each driver fills the shape, material,
+// light and camera gradients itself.
+inline const char* setup_backward(const rb_dscene_desc& d_scene, const DevScene& sc, const rb_texture* emission, KernelArgs& ka) {
     if (d_scene.num_shapes != sc.num_shapes || d_scene.num_materials != sc.num_materials || d_scene.num_lights != sc.num_lights - (sc.has_envmap ? 1 : 0))
         return "rb_render: d_scene does not match the scene (shape / material / light counts)";
+    if (const char* err = check_light_emission_grads(d_scene, emission)) return err;
     if (boundary_stage_runs(sc, ka.rp) && ka.rp.max_bounces > RB_MAX_BOUNDARY_BOUNCES) return "rb_render: secondary edge sampling supports at most 64 bounces";
     memset(&ka.ds.env_values, 0, sizeof(rb_texture));
     ka.ds.env_w2e = nullptr;
@@ -525,7 +540,19 @@ RB_D void bwd_sweep(const DevScene& sc, const KernelArgs& ka, int pixel, int px,
         {
             const rb_shape& shape = sc.shapes[is.shape_id];
             V3 wi = -ray.dir;
-            if (shape.light_id >= 0 && dot(wi, sp.shading_frame.n) > 0) {
+            if (shape.light_id >= 0 && RB_LIGHT_TEX(light_emission(sc, shape.light_id))) {
+                // An emission texture: under the forward's condition (the untextured branch below keeps the reference's gate), into the
+                // intensity, the texture, and through d(uv) and the footprint into the hit (DESIGN.md "Emission textures").
+                const DevLight& light = sc.lights[shape.light_id];
+                if (light.directly_visible && (light.two_sided || dot(wi, sp.shading_frame.n) > 0)) {
+                    const V3 I = mk3(light.intensity[0], light.intensity[1], light.intensity[2]);
+                    agg_add3(ds.light_intensity[shape.light_id], d_emission * light_tex_eval(light_emission(sc, shape.light_id), sp.uv, sp.du_dxy, sp.dv_dxy));
+                    V2 d_du = zero2(), d_dv = zero2();
+                    adj.d_point.uv += d_light_tex_eval(sc, ds, shape.light_id, sp.uv, sp.du_dxy, sp.dv_dxy, d_emission * I, d_du, d_dv);
+                    adj.d_point.du_dxy += d_du;
+                    adj.d_point.dv_dxy += d_dv;
+                }
+            } else if (shape.light_id >= 0 && dot(wi, sp.shading_frame.n) > 0) {
                 const DevLight& light = sc.lights[shape.light_id];
                 if (light.directly_visible) agg_add3(ds.light_intensity[shape.light_id], d_emission);
             }

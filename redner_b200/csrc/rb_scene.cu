@@ -491,6 +491,8 @@ static int scene_apply(rb_scene* sc, const rb_scene_desc& desc, bool geometry, b
     sc->shapes.assign(desc.shapes, desc.shapes + desc.num_shapes);
     sc->materials.assign(desc.materials, desc.materials + desc.num_materials);
     sc->lights = host_area_lights(desc);
+    sc->light_emission = host_light_emission(desc);
+    sc->light_table = light_table_words(sc->lights.data(), sc->light_emission.data(), (int)sc->lights.size());
     host_setup_envmap(desc.envmap, sc->dev);
     rb_shape* d_shapes;
     rb_material* d_materials;
@@ -668,6 +670,7 @@ extern "C" int rb_scene_table(const rb_scene* sc, int which, void* out, size_t b
         case RB_TABLE_AREA_CDF_OFFSETS: src = d.area_cdf_offset; n = sizeof(int) * (size_t)L; break;
         case RB_TABLE_PRIMARY_EDGE_PMF: src = d.prim_edge_pmf; n = prim ? sizeof(double) * (size_t)d.num_edges : 0; break;
         case RB_TABLE_PRIMARY_EDGE_CDF: src = d.prim_edge_cdf; n = prim ? sizeof(double) * (size_t)d.num_edges : 0; break;
+        case RB_TABLE_LIGHTS: src = d.lights; n = L > 0 ? sizeof(unsigned long long) * sc->light_table.size() : 0; break;
         default: rb_set_error("rb_scene_table: unknown table"); return 1;
     }
     if (src == nullptr || (d.num_lights == 0 && which >= RB_TABLE_LIGHT_PMF && which <= RB_TABLE_AREA_CDF_OFFSETS)) n = 0;

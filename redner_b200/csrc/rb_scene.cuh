@@ -48,6 +48,8 @@ struct rb_scene {
     std::vector<rb_shape> shapes;
     std::vector<rb_material> materials;
     std::vector<DevLight> lights;
+    std::vector<rb_texture> light_emission;      // per area light: its emission texture (num_levels == 0: none)
+    std::vector<unsigned long long> light_table; // what SS_LIGHTS holds: the DevLights, then the emission textures (light_emission)
     std::vector<int> light_offsets; // [lights + 1]: first entry of every light in the area-CDF pool, then the pool size
     int max_generic_texture_dimension = 0;
     int has_envmap = 0;

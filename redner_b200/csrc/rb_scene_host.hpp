@@ -65,14 +65,29 @@ inline void host_setup_pixel_filter(const rb_pixel_filter& f, DevCamera& dc) {
     dc.filter_type = g.type;
     dc.filter_width = g.width;
 }
-// Index, pixel-filter and specular-model checks of the descriptor; returns the error message, or null.
+// An area light's emission texture (rb_area_light::emission); returns the error message, or null.
+inline const char* host_check_emission(const rb_texture& t) {
+    if (t.num_levels == 0) return nullptr;
+    if (t.num_levels < 0 || t.num_levels > RB_MAX_MIP_LEVELS) return "rb_scene_create: a light's emission texture needs num_levels in [0, RB_MAX_MIP_LEVELS]";
+    if (t.channels != 1 && t.channels != 3) return "rb_scene_create: a light's emission texture needs 1 or 3 channels";
+    if (t.uv_scale == nullptr) return "rb_scene_create: a light's emission texture needs a uv_scale";
+    const bool constant = t.width[0] == 0 && t.height[0] == 0;
+    for (int k = 0; k < t.num_levels; k++) {
+        if (t.texels[k] == nullptr) return "rb_scene_create: a level of a light's emission texture has no texels";
+        if (!constant && (t.width[k] <= 0 || t.height[k] <= 0)) return "rb_scene_create: a level of a light's emission texture needs a positive size";
+    }
+    return nullptr;
+}
+// Index, pixel-filter, specular-model and emission-texture checks of the descriptor; returns the error message, or null.
 inline const char* host_check_scene_desc(const rb_scene_desc& desc) {
     if (const char* err = host_check_pixel_filter(desc)) return err;
     for (int m = 0; m < desc.num_materials; m++)
         if (desc.materials[m].specular_model != RB_SPECULAR_BLINN_PHONG && desc.materials[m].specular_model != RB_SPECULAR_GGX)
             return "rb_scene_create: material specular_model must be RB_SPECULAR_BLINN_PHONG (0) or RB_SPECULAR_GGX (1)";
-    for (int l = 0; l < desc.num_lights; l++)
+    for (int l = 0; l < desc.num_lights; l++) {
         if (desc.lights[l].shape_id < 0 || desc.lights[l].shape_id >= desc.num_shapes) return "rb_scene_create: area light refers to an invalid shape";
+        if (const char* err = host_check_emission(desc.lights[l].emission)) return err;
+    }
     for (int s = 0; s < desc.num_shapes; s++) {
         const rb_shape& sh = desc.shapes[s];
         if (sh.material_id < 0 || sh.material_id >= desc.num_materials) return "rb_scene_create: shape refers to an invalid material";
@@ -90,6 +105,12 @@ inline std::vector<DevLight> host_area_lights(const rb_scene_desc& desc) {
         dl.directly_visible = desc.lights[l].directly_visible;
         out.push_back(dl);
     }
+    return out;
+}
+// The lights' emission textures (one per area light, num_levels == 0: none).
+inline std::vector<rb_texture> host_light_emission(const rb_scene_desc& desc) {
+    std::vector<rb_texture> out;
+    for (int l = 0; l < desc.num_lights; l++) out.push_back(desc.lights[l].emission);
     return out;
 }
 inline int host_max_generic_texture_dimension(const rb_scene_desc& desc) {

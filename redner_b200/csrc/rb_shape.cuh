@@ -172,6 +172,12 @@ RB_HD void tri_attribs(const rb_shape& s, int t, TriAttribs& a) {
         a.uv2 = mk2(1, 1);
     }
 }
+// Texture coordinate at barycentrics (u, v) of a triangle (weights 1 - u - v, u, v of its corners): the uv of a ray hit
+// (make_surface_point) and of a light sample (light_sample_uv) alike.
+RB_HD V2 tri_uv(const TriAttribs& a, Real u, Real v) {
+    Real w = 1 - (u + v);
+    return w * a.uv0 + u * a.uv1 + v * a.uv2;
+}
 RB_HD V3 shape_normal(const rb_shape& s, int i) {
     const float* p = s.normals + 3 * (size_t)i;
     return mk3(p[0], p[1], p[2]);
@@ -188,7 +194,7 @@ RB_HD SurfacePoint make_surface_point(const rb_shape& s, int tri, const Ray& ray
     TriSolve h = tri_solve(v0, v1, v2, ray, rd);
     Real u = h.u, v = h.v, w = 1 - (u + v), t = h.t;
     SurfacePoint p;
-    p.uv = w * a.uv0 + u * a.uv1 + v * a.uv2;
+    p.uv = tri_uv(a, u, v);
     // hit point: product and sum rounded separately like the reference's (src/shape.h:295), see rb_mul_add_unfused
     p.position = mk3(rb_mul_add_unfused(ray.dir.x, t, ray.org.x), rb_mul_add_unfused(ray.dir.y, t, ray.org.y), rb_mul_add_unfused(ray.dir.z, t, ray.org.z));
     V3 gn = normalize(cross(v1 - v0, v2 - v0));
@@ -479,4 +485,12 @@ RB_HD void d_sample_light_triangle(const rb_shape& s, int tri, V2 sample, const 
     d_v[0] += d_v0;
     d_v[1] += d_e1;
     d_v[2] += d_e2;
+}
+// Texture coordinate of the light sample `sample` on triangle `tri` (sample_light_triangle keeps the sample itself in
+// SurfacePoint::uv): the hit's interpolation at the sample's barycentrics.  It depends on the uv vertices only, not on the positions.
+RB_HD V2 light_sample_uv(const rb_shape& s, int tri, V2 sample) {
+    TriAttribs a;
+    tri_attribs(s, tri, a);
+    Real r = sqrt(sample.x);
+    return tri_uv(a, 1 - r, r * sample.y);
 }

@@ -1,5 +1,8 @@
 // Device-side scene description shared by all kernels.
 #pragma once
+#include <cstring>
+#include <vector>
+
 #include "../../include/redner_b200.h"
 #include "rb_math.cuh"
 
@@ -180,6 +183,38 @@ struct DevDScene {
     // [0..15] d_cam_to_world, [16..31] d_world_to_cam, [32..40] d_intrinsic_mat_inv, [41..49] d_intrinsic_mat, ... (CamAcc, rb_camera.cuh)
     double* cam_accum;
 };
+
+// Emission textures of the area lights (rb_area_light::emission) and their gradients sit in tables of their own, so that DevLight,
+// DevScene and DevDScene keep the layout the lean and diffuse-only kernels are compiled against.  The scene's table follows its DevLight
+// array in the same allocation; the gradient table of a backward pass follows the array of intensity-gradient pointers that
+// DevDScene::light_intensity points at.  Each starts at the first 16-byte boundary after its array and holds one rb_texture per area
+// light (num_levels == 0: no texture, or no gradient).  Only kernels with RB_LIGHT_TEX read them.
+RB_HD size_t light_table_offset(size_t array_bytes) { return (array_bytes + 15) & ~(size_t)15; }
+RB_HD int num_area_lights(const DevScene& sc) { return sc.num_lights - (sc.has_envmap ? 1 : 0); }
+RB_HD const rb_texture& light_emission(const DevScene& sc, int l) {
+    return ((const rb_texture*)((const char*)sc.lights + light_table_offset((size_t)num_area_lights(sc) * sizeof(DevLight))))[l];
+}
+RB_HD const rb_texture& light_d_emission(const DevScene& sc, const DevDScene& ds, int l) {
+    return ((const rb_texture*)((const char*)ds.light_intensity + light_table_offset((size_t)num_area_lights(sc) * sizeof(float*))))[l];
+}
+// Host image of such a table: the n entries of `head`, then the n textures of `tex` (zeroed when `tex` is null), in 8-byte words.
+template <typename T>
+inline std::vector<unsigned long long> light_table_words(const T* head, const rb_texture* tex, int n) {
+    const size_t off = light_table_offset((size_t)n * sizeof(T));
+    std::vector<unsigned long long> w((off + (size_t)n * sizeof(rb_texture) + 7) / 8, 0ull);
+    if (n > 0) {
+        memcpy(w.data(), head, (size_t)n * sizeof(T));
+        if (tex) memcpy((char*)w.data() + off, tex, (size_t)n * sizeof(rb_texture));
+    }
+    return w;
+}
+// True when some light has an emission texture (RB_LIGHT_TEX), i.e. when only the general and deterministic kernels compute what the
+// scene asks for.
+inline bool lights_use_emission(const std::vector<rb_texture>& emission) {
+    for (const rb_texture& t : emission)
+        if (t.num_levels > 0) return true;
+    return false;
+}
 
 struct RenderParams {
     unsigned long long seed;

@@ -253,18 +253,24 @@ class DMaterial:  # src/redner.cpp:153-158
 
 
 class AreaLight:  # src/redner.cpp:160-164, src/area_light.h:8-36
-    def __init__(self, shape_id, intensity, two_sided, directly_visible):
+    def __init__(self, shape_id, intensity, two_sided, directly_visible, emission=None):
+        """`emission` (redner_b200 extension): a Texture1 or Texture3, the light's emission texture (rb_area_light::emission), or None."""
         a = L.rb_area_light()
         a.shape_id = int(shape_id)
         a.intensity[:] = _read_floats(intensity, 3)
         a.two_sided = int(bool(two_sided))
         a.directly_visible = int(bool(directly_visible))
+        if emission is not None:
+            a.emission = emission._c
         self._c = a
 
 
 class DAreaLight:  # src/redner.cpp:166-167
-    def __init__(self, intensity):
+    def __init__(self, intensity, emission=None):
+        """`emission` (redner_b200 extension): the gradient pyramid of the light's emission texture (a Texture1 / Texture3 of its shape), or
+        None."""
         self.addr = _addr(intensity)
+        self.emission = emission
 
 
 class EnvironmentMap:  # src/redner.cpp:169-178
@@ -575,6 +581,12 @@ class DScene:  # src/redner.cpp:75-82
         d.num_shapes, d.shapes = len(shapes), self._shapes
         d.num_materials, d.materials = len(materials), self._materials
         d.num_lights, d.light_intensity = len(area_lights), self._lights
+        # (the emission gradients only when some light has one: otherwise the descriptor is the one without emission textures)
+        emission = [getattr(a, "emission", None) for a in area_lights]
+        self._emission = None
+        if any(e is not None for e in emission):
+            self._emission = (L.rb_texture * len(area_lights))(*[e._c if e is not None else L.rb_texture() for e in emission])
+            d.light_emission = self._emission
         self.envmap = envmap
         d.envmap = C.pointer(envmap._c) if envmap is not None else None
         self._c = d

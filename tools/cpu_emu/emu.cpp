@@ -23,6 +23,8 @@ struct rb_scene {
     std::vector<rb_shape> shapes;
     std::vector<rb_material> materials;
     std::vector<DevLight> lights;
+    std::vector<rb_texture> light_emission;      // per area light (num_levels == 0: none)
+    std::vector<unsigned long long> light_table; // what the kernels read at dev.lights: the DevLights, then light_emission
     HostLightTables lt;
     HostEdgeTables et;
     HostEdgeTree tree;
@@ -98,6 +100,8 @@ static int emu_build(rb_scene* sc, const rb_scene_desc* desc) {
     sc->shapes.assign(desc->shapes, desc->shapes + desc->num_shapes);
     sc->materials.assign(desc->materials, desc->materials + desc->num_materials);
     sc->lights = host_area_lights(*desc);
+    sc->light_emission = host_light_emission(*desc);
+    sc->light_table = light_table_words(sc->lights.data(), sc->light_emission.data(), (int)sc->lights.size());
     sc->max_generic = host_max_generic_texture_dimension(*desc);
     d.edge_root_cs = d.edge_root_ncs = RB_EDGE_EMPTY;
     d.shapes = sc->shapes.data();
@@ -152,7 +156,7 @@ static int emu_build(rb_scene* sc, const rb_scene_desc* desc) {
     d.num_lights = (int)sc->lights.size() + (d.has_envmap ? 1 : 0);
     if (d.num_lights > 0) {
         if (!host_build_lights(sc->lights, meshes, sc->lt, g_err, d.has_envmap != 0, d.has_envmap ? desc->envmap->pdf_norm : 0.0, host_bsphere_radius(meshes))) return 1;
-        d.lights = sc->lights.data();
+        d.lights = (const DevLight*)sc->light_table.data();
         d.light_pmf = sc->lt.pmf.data();
         d.light_cdf = sc->lt.cdf.data();
         d.light_areas = sc->lt.areas.data();
@@ -231,6 +235,7 @@ extern "C" int rb_scene_table(const rb_scene* sc, int which, void* out, size_t b
         case RB_TABLE_AREA_CDF_OFFSETS: src = sc->lt.offsets.data(); n = lights ? sizeof(int) * sc->lt.offsets.size() : 0; break;
         case RB_TABLE_PRIMARY_EDGE_PMF: src = sc->et.prim_pmf.data(); n = prim ? sizeof(double) * (size_t)d.num_edges : 0; break;
         case RB_TABLE_PRIMARY_EDGE_CDF: src = sc->et.prim_cdf.data(); n = prim ? sizeof(double) * (size_t)d.num_edges : 0; break;
+        case RB_TABLE_LIGHTS: src = sc->light_table.data(); n = sc->lights.empty() ? 0 : sizeof(unsigned long long) * sc->light_table.size(); break;
         default: g_err = "rb_scene_table: unknown table"; return 1;
     }
     if (size) *size = n;
@@ -464,6 +469,10 @@ static int emu_render(const rb_scene* scene, const rb_options* opt, float* image
         g_err = "rb_render: this build has no thin lens (lens_radius)";
         return 1;
     }
+    if (lights_use_emission(scene->light_emission)) {
+        g_err = "rb_render: this build has no emission textures (rb_area_light::emission)";
+        return 1;
+    }
 #endif
     const DevScene& sc = scene->dev;
     if (image && !rp.only_radiance) {
@@ -489,7 +498,7 @@ static int emu_render(const rb_scene* scene, const rb_options* opt, float* image
             }
     }
     if (d_image) {
-        if (const char* err = setup_backward(*d_scene, sc, ka)) {
+        if (const char* err = setup_backward(*d_scene, sc, scene->light_emission.data(), ka)) {
             g_err = err;
             return 1;
         }
@@ -498,7 +507,8 @@ static int emu_render(const rb_scene* scene, const rb_options* opt, float* image
         std::vector<float> cam_f(n_cam, 0.f);
         ka.ds.shapes = d_scene->shapes;
         ka.ds.materials = d_scene->materials;
-        ka.ds.light_intensity = d_scene->light_intensity;
+        std::vector<unsigned long long> light_grads = light_table_words(d_scene->light_intensity, d_scene->light_emission, d_scene->num_lights);
+        ka.ds.light_intensity = (float* const*)light_grads.data();
         ka.ds.cam_accum = cam_accum.data();
         CamAcc acc;
         acc.base = cam_f.data();
@@ -517,7 +527,7 @@ static int emu_render(const rb_scene* scene, const rb_options* opt, float* image
                 for (long long i = 0; i <= xl.num_acc; i++) exact_normalise(&xacc[(size_t)i * RB_EXACT_WORDS]);
         };
         if (det) {
-            exact_layout(*d_scene, scene->shapes.data(), scene->materials.data(), sc, ka, xl);
+            exact_layout(*d_scene, scene->shapes.data(), scene->materials.data(), scene->light_emission.data(), sc, ka, xl);
             if (records && xl.overlaps) {
                 g_err = "rb_render_exact: gradient buffers of d_scene overlap; records need disjoint buffers";
                 return 1;
@@ -530,7 +540,8 @@ static int emu_render(const rb_scene* scene, const rb_options* opt, float* image
             xacc.assign((size_t)(xl.num_acc + 1) * RB_EXACT_WORDS, 0);
             ka.ds.shapes = xl.shapes.data();
             ka.ds.materials = xl.materials.data();
-            ka.ds.light_intensity = xl.lights.data();
+            light_grads = light_table_words(xl.lights.data(), xl.light_emission.empty() ? nullptr : xl.light_emission.data(), d_scene->num_lights);
+            ka.ds.light_intensity = (float* const*)light_grads.data();
             ka.ds.env_values = xl.env_values;
             ka.ds.env_w2e = xl.env_w2e;
             ka.screen_grad = xl.screen_grad;
@@ -598,7 +609,7 @@ extern "C" int rb_exact_record_count(const rb_scene* scene, const rb_options* op
     ExactLayout xl;
     std::string err;
     if (const char* e = exact_record_layout("rb_exact_record_count", *opt, scene->cam, scene->max_generic, d_scene, screen_grad, scene->shapes.data(),
-                                            scene->materials.data(), scene->dev, ka, xl, err)) {
+                                            scene->materials.data(), scene->light_emission.data(), scene->dev, ka, xl, err)) {
         g_err = e;
         return 1;
     }
@@ -628,7 +639,7 @@ extern "C" int rb_exact_round(const rb_scene* scene, const rb_options* opt, cons
     ExactLayout xl;
     std::string err;
     if (const char* e = exact_record_layout("rb_exact_round", *opt, scene->cam, scene->max_generic, d_scene, screen_grad, scene->shapes.data(),
-                                            scene->materials.data(), scene->dev, ka, xl, err)) {
+                                            scene->materials.data(), scene->light_emission.data(), scene->dev, ka, xl, err)) {
         g_err = e;
         return 1;
     }
