@@ -117,12 +117,25 @@ typedef struct rb_area_light {
      * shape, where E is this 1- or 3-channel mip-mapped texture (1 channel is broadcast to RGB) and uv the shape's texture coordinate there
      * (its uvs, or the default per-triangle uvs, times uv_scale).  Rays from the camera and edge rays look it up with the footprint of the
      * material textures at that hit; light samples and BSDF-sampled hits with a zero footprint.  Light selection and the point on the
-     * light are sampled as without a texture.  rb_scene_create and rb_scene_update refuse, with a message naming the emission texture, a
+     * light are sampled as without a texture unless emission_sampling asks otherwise.  rb_scene_create and rb_scene_update refuse, with a message naming the emission texture, a
      * channel count other than 1 or 3, num_levels outside [0, RB_MAX_MIP_LEVELS], a level without texels, a non-constant level without a
      * positive size and a missing uv_scale.  rb_scene_update may add, change or remove the texture: it is a value of the light, like
      * intensity. */
     rb_texture emission;
+    /* One of rb_emission_sampling, below (no reference counterpart; DESIGN.md "Emission sampling").  RB_EMISSION_SAMPLE_AREA (the zero-initialised field)
+     * places light samples uniformly by area, as the reference does.  RB_EMISSION_SAMPLE_TEXTURE, on a light whose emission texture is not
+     * constant, places them by a defensive mixture: with probability 1/8 uniformly by area, otherwise by the luminance of the texture's
+     * level 0 (a triangle by its area times the mean cell weight over its uv bounding box, then a texel cell, then a point uniformly in
+     * the cell; a point outside the triangle is rejected and contributes nothing).  The light's selection weight then uses the sum of
+     * those triangle weights in place of its area.  Without a texture, or with a constant one, the option changes nothing.  The tables
+     * are rebuilt from the texels by every rb_scene_create and rb_scene_update; texels written in place without an update leave them
+     * stale, which costs variance but no bias.  rb_scene_create and rb_scene_update refuse, with a message naming the emission sampling,
+     * any other value and a light whose scaled texture coordinates (uv * uv_scale * level-0 size) reach 2^24 cells in magnitude or are
+     * not finite. */
+    int emission_sampling;
 } rb_area_light;
+/* rb_area_light::emission_sampling */
+enum rb_emission_sampling { RB_EMISSION_SAMPLE_AREA = 0, RB_EMISSION_SAMPLE_TEXTURE = 1 };
 
 /* EnvironmentMap -- src/envmap.h:19-51, constructor src/redner.cpp:169-178.  `values` is the [h, w, 3] mip pyramid, the two
  * tables are the caller's importance-sampling CDFs (pyredner/envmap.py:36-61); all device memory, matrices row-major. */
@@ -247,7 +260,8 @@ int rb_scene_create_on_stream(const rb_scene_desc* desc, rb_scene** out, void* s
  * Any pointer may change, and so may every value passed by value (camera, light intensities, the environment map's matrices and
  * pdf_norm).
  * The build reads vertex positions in place, so an in-place write to them is invisible to the library: pass geometry_changed != 0
- * after one.  Then -- or when any `vertices` pointer changed -- the BVH, the light areas and area CDFs, the environment map's
+ * after one.  Texels are read in place too: the emission-sampling tables (rb_area_light::emission_sampling) are rebuilt from them by every
+ * update, and an in-place texel write without one leaves them stale, which keeps the image unbiased but noisier.  Then -- or when any `vertices` pointer changed -- the BVH, the light areas and area CDFs, the environment map's
  * bounding sphere, the edge list and the camera-dependent tables are rebuilt.  Otherwise, when the camera or the pixel filter differs by
  * value, only the camera-dependent tables are, as rb_scene_set_camera does (but on the host for the small scenes whose build made them there, so
  * that they stay the build's tables byte for byte).  The shape / material descriptors, the lights and the light PMF / CDF are
@@ -363,8 +377,12 @@ enum rb_scene_table_id {
     RB_TABLE_AREA_CDF_OFFSETS,   /* int per area light: first entry in the pool */
     RB_TABLE_PRIMARY_EDGE_PMF,   /* double per edge (src/edge.cpp:298-331); empty without primary-edge sampling */
     RB_TABLE_PRIMARY_EDGE_CDF,
-    RB_TABLE_LIGHTS              /* the area lights as the kernels read them: { shape_id, intensity, two_sided, directly_visible } per light
+    RB_TABLE_LIGHTS,             /* the area lights as the kernels read them: { shape_id, intensity, two_sided, directly_visible } per light
                                     (24 bytes), then from the next 16-byte boundary the lights' emission textures (rb_texture each) */
+    RB_TABLE_LIGHT_SAMPLING      /* doubles, for every light that samples by its emission texture (RB_EMISSION_SAMPLE_TEXTURE with a texture
+                                    that is not constant), in light order: { S, 0 } (S: the sum of the triangle weights a_t), the w x h cell
+                                    weights of level 0 (row-major), their w x h summed-area table, then per triangle { x0, y0, x1, y1, M_t,
+                                    a_t, CDF_t, pdf factor } (DESIGN.md "Emission sampling"); empty when no light does */
 };
 int rb_scene_table(const rb_scene* scene, int which, void* out, size_t bytes, size_t* size);
 
@@ -404,6 +422,16 @@ int rb_texture_test(const rb_texture* tex, const rb_texture* d_tex, const float*
  * Runs on `stream` (a cudaStream_t, NULL == legacy default stream) and synchronises it. */
 int rb_envmap_test(const rb_envmap* env, const rb_texture* d_values, float* d_w2e, const float* queries, int n, const float* d_out, float* values,
                    float* pdfs, float* d_queries, const double* samples, int m, float* sample_dirs, void* stream);
+
+/* Test hook: the point-on-light sampler and its density for area light `light` of a built scene, through the functions the render
+ * kernels call (rb_path.cuh).  samples: [n, 3] doubles (tri_sel, su, sv); ints receives [n, 3] { branch (0: by area, 1: by texture),
+ * triangle, rejected }; doubles receives [n, 3] { b1, b2, density }, where (b1, b2) are the barycentrics of the point as the light-sample
+ * record reproduces it and density the area density of that point evaluated from the record (0 for a rejected sample).  queries: [m, 3]
+ * floats { triangle, u, v } (u, v: the light's texture coordinate before uv_scale); query_pdfs receives the area density at each.  The
+ * densities do not include the light-selection probability; a query whose triangle is out of range gets NaN.  Every buffer is memory of
+ * the scene's device; a light out of range and a negative count are refused.  Runs on `stream` and synchronises it. */
+int rb_light_sample_test(const rb_scene* scene, int light, const double* samples, int n, int* ints, double* doubles, const float* queries, int m,
+                         double* query_pdfs, void* stream);
 
 const char* rb_last_error(void);
 const char* rb_version(void);

@@ -174,11 +174,18 @@ class Shape:
 class AreaLight:
     """`emission` (redner_b200 extension): None, or the light's emission texture, a Texture or an [h, w, 1 | 3] (or [1 | 3] constant) float32
     tensor that may require grad.  The light then emits intensity * E(uv) at a point of its shape whose texture coordinate is uv
-    (DESIGN.md "Emission textures")."""
+    (DESIGN.md "Emission textures").  `emission_sampling` (redner_b200 extension): "area" places light samples uniformly by area;
+    "texture" places most of them by the emission texture's luminance (DESIGN.md "Emission sampling"), which leaves the expected image and
+    gradients as they are and cuts the noise of lights whose emission is concentrated in part of their surface."""
+    EMISSION_SAMPLING = ("area", "texture")  # rb_emission_sampling
 
-    def __init__(self, shape_id: int, intensity: torch.Tensor, two_sided: bool = False, directly_visible: bool = True, emission=None):
+    def __init__(self, shape_id: int, intensity: torch.Tensor, two_sided: bool = False, directly_visible: bool = True, emission=None,
+                 emission_sampling: str = "area"):
         assert intensity.dtype == torch.float32 and tuple(intensity.shape) == (3,)
+        if emission_sampling not in self.EMISSION_SAMPLING:
+            raise ValueError("AreaLight: emission_sampling must be one of %s, not %r" % (", ".join(self.EMISSION_SAMPLING), emission_sampling))
         self.shape_id, self.intensity, self.two_sided, self.directly_visible = shape_id, intensity, two_sided, directly_visible
+        self.emission_sampling = emission_sampling
         self.emission = _as_texture(emission)
         if self.emission is not None:
             t = self.emission.texels
@@ -237,7 +244,8 @@ _MaterialArgs = namedtuple("_MaterialArgs", "textures compute_specular_lighting 
 _LightArgs = namedtuple("_LightArgs", "shape_id intensity two_sided directly_visible")
 _EnvmapArgs = namedtuple("_EnvmapArgs", "values env_to_world world_to_env sample_cdf_ys sample_cdf_xs pdf_norm directly_visible")
 _OptionArgs = namedtuple("_OptionArgs", "num_samples max_bounces channels sampler_type use_primary_edge_sampling use_secondary_edge_sampling "
-                                        "sample_pixel_center pixel_filter device backend specular_models lens_radius focus_distance light_emission")
+                                        "sample_pixel_center pixel_filter device backend specular_models lens_radius focus_distance light_emission "
+                                        "emission_sampling")
 
 
 def _ptr(backend, t, kind="float"):
@@ -396,6 +404,9 @@ class RenderFunction(torch.autograd.Function):
                     args.pop(-2 - len(t.mipmap))  # (the level count is in the tuple)
         else:
             args.append(None)
+        # the lights' rb_emission_sampling values, None when every one is "area" (the very last entry, so that no other one moves)
+        sampling = tuple(AreaLight.EMISSION_SAMPLING.index(getattr(light, "emission_sampling", "area")) for light in scene.area_lights)
+        args.append(sampling if any(sampling) else None)
         return args
 
     @staticmethod
@@ -444,8 +455,9 @@ class RenderFunction(torch.autograd.Function):
         if values is not None:
             rest, rest_pos = entries(len(_EnvmapArgs._fields) - 1)
             a.env_args, a.pos.env_args = _EnvmapArgs(values, *rest), _EnvmapArgs(positions, *rest_pos)
-        a.option_args, a.pos.option_args = take(_OptionArgs)
-        levels = a.option_args.light_emission or (0,) * args[2]
+        # (the options up to light_emission, then the emission textures that entry announces, then emission_sampling: the list's last entry)
+        values, positions = entries(len(_OptionArgs._fields) - 1)
+        levels = values[-1] or (0,) * args[2]
         a.emission_args, a.pos.emission_args = [], []
         for n in levels:
             t, q = None, None
@@ -454,6 +466,8 @@ class RenderFunction(torch.autograd.Function):
                 t, q = _TextureArgs(list(mips), uv[0]), _TextureArgs(list(mip_pos), uv_pos[0])
             a.emission_args.append(t)
             a.pos.emission_args.append(q)
+        sampling, sampling_pos = entries(1)
+        a.option_args, a.pos.option_args = _OptionArgs(*values, *sampling), _OptionArgs(*positions, *sampling_pos)
         assert k == len(args), "serialize_scene's list has %d entries, its layout %d" % (len(args), k)
         return a
 
@@ -488,8 +502,11 @@ class RenderFunction(torch.autograd.Function):
             materials.append(rb.Material(*textures, m.compute_specular_lighting, m.two_sided, m.use_vertex_color,
                                          **({} if models is None or not models[i] else {"specular_model": models[i]})))
         # (the keyword only for a textured light: a backend without emission textures renders the others)
+        # (and emission_sampling only when some light samples by its texture)
+        sampling = c.option_args.emission_sampling or (0,) * len(c.light_args)
         lights = [rb.AreaLight(l.shape_id, fp(l.intensity), l.two_sided, l.directly_visible,
-                               **({} if e is None else {"emission": _native_texture(rb, rb.TextureN, 0, e)})) for l, e in zip(c.light_args, c.emission_args)]
+                               **({} if e is None else {"emission": _native_texture(rb, rb.TextureN, 0, e)}),
+                               **({} if not es else {"emission_sampling": int(es)})) for l, e, es in zip(c.light_args, c.emission_args, sampling)]
         envmap = None
         if c.env_args is not None:
             e = c.env_args

@@ -15,11 +15,13 @@
 
 #include "rb_light_build.cuh"
 #include "rb_scene.cuh"
+#include "rb_scene_host.hpp"
 
 // persistent per scene (slot SS_LIGHT_AUX): the vertex bounds survive updates that do not move vertices
 struct LightAux {
     unsigned int bounds[4]; // lo x, lo y, hi x, hi y as order-preserving integers
     int status;             // 1: the total light importance is not positive
+    int uv_status;          // 1: a light's scaled texture coordinates are out of the range of emission sampling (RB_LS_MAX_CELLS)
 };
 
 __device__ __forceinline__ unsigned int lt_f2ord(float f) {
@@ -80,9 +82,64 @@ __global__ void k_lt_bounds(const rb_shape* shapes, int num_shapes, LightAux* au
             atomicMax(&aux->bounds[2 + a], lt_f2ord(hi[a]));
         }
 }
-__global__ void k_lt_pmf(const DevLight* lights, int L, const double* areas, int has_env, int num_shapes, double pdf_norm, LightAux* aux, double* pmf,
-                         double* cdf) {
-    for (int l = 0; l < L; l++) pmf[l] = lt_light_weight(lights[l], areas[l]);
+// ---- emission sampling (the ls_* steps of rb_light_build.cuh), per light that samples by its texture
+//   k_ls_cells    one thread per cell: its weight
+//   k_ls_rows     one thread per row: prefix sums along it; then k_ls_cols, one thread per column: prefix sums down it
+//   k_ls_tris     one thread per triangle: its record (R_t, M_t, a_t, |T_t| / (M_t area_t)); flags coordinates out of range
+//   k_ls_scan     one warp: S, the CDF of a_t and the pdf factors, with ls_scan's additions in its order (as k_lt_scan does it)
+__global__ void k_ls_cells(rb_texture t, double* d) {
+    const int w = t.width[0], h = t.height[0];
+    const long long c = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+    if (c < (long long)w * h) d[ls_cells(w, h) + c] = ls_cell_weight(t.texels[0], t.channels, w, h, (int)(c % w), (int)(c / w));
+}
+__global__ void k_ls_rows(int w, int h, double* d) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j < h) ls_sat_row(d + ls_cells(w, h), d + ls_sat(w, h), w, j);
+}
+__global__ void k_ls_cols(int w, int h, double* d) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < w) ls_sat_col(d + ls_sat(w, h), w, h, i);
+}
+__global__ void k_ls_tris(const rb_shape* shapes, int shape_id, rb_texture t, double* d, LightAux* aux) {
+    const rb_shape& sh = shapes[shape_id];
+    const int k = blockIdx.x * blockDim.x + threadIdx.x, w = t.width[0], h = t.height[0];
+    if (k < sh.num_triangles && !ls_tri_record(sh, k, t.uv_scale[0], t.uv_scale[1], w, h, d + ls_sat(w, h), d + ls_tris(w, h) + RB_LS_TRI * (size_t)k))
+        aux->uv_status = 1;
+}
+__global__ void k_ls_scan(int T, int w, int h, double* d) {
+    const int lane = threadIdx.x & 31;
+    double* recs = d + ls_tris(w, h);
+    double sum = 0;
+    for (int t0 = 0; t0 < T; t0 += 32) {
+        const double v = t0 + lane < T ? recs[RB_LS_TRI * (size_t)(t0 + lane) + 5] : 0.0;
+        const int n = min(32, T - t0);
+        for (int j = 0; j < n; j++) sum += __shfl_sync(0xffffffffu, v, j);
+    }
+    double run = 0;
+    for (int t0 = 0; t0 < T; t0 += 32) {
+        const double v = t0 + lane < T ? recs[RB_LS_TRI * (size_t)(t0 + lane) + 5] : 0.0;
+        const int n = min(32, T - t0);
+        double mine = 0;
+        for (int j = 0; j < n; j++) {
+            if (lane == j) mine = run;
+            run += __shfl_sync(0xffffffffu, v, j);
+        }
+        if (t0 + lane < T) {
+            double* r = recs + RB_LS_TRI * (size_t)(t0 + lane);
+            r[6] = sum > 0 ? mine / sum : 0.0;
+            r[7] = sum > 0 ? (v / sum) * r[7] : 0.0;
+        }
+    }
+    if (lane == 0) {
+        d[0] = sum;
+        d[1] = 0;
+    }
+}
+
+// sel: the descriptors of the lights' emission sampling (null when no light uses it); a light with S > 0 is selected by S instead of its area
+__global__ void k_lt_pmf(const DevLight* lights, int L, const double* areas, const LightSampling* sel, int has_env, int num_shapes, double pdf_norm, LightAux* aux,
+                         double* pmf, double* cdf) {
+    for (int l = 0; l < L; l++) pmf[l] = lt_light_weight(lights[l], sel && sel[l].data ? ls_selection_area(areas[l], sel[l].data[0]) : areas[l]);
     if (has_env) {
         double radius = 0;
         if (num_shapes > 0) {
@@ -112,7 +169,7 @@ int rb_build_lights(rb_scene* sc, bool geometry, cudaStream_t stream) {
         scene_table(sc, SS_LIGHT_CDF, sc->dev.num_lights, stream, &d_cdf) || scene_table(sc, SS_LIGHT_AUX, 1, stream, &aux))
         return 1;
     d_lights = (DevLight*)d_table;
-    if (L > 0) RB_CUDA_OK(cudaMemcpyAsync(d_table, sc->light_table.data(), sizeof(unsigned long long) * sc->light_table.size(), cudaMemcpyHostToDevice, stream));
+    RB_CUDA_OK(cudaMemcpyAsync(d_table, sc->light_table.data(), sizeof(unsigned long long) * sc->light_table.size(), cudaMemcpyHostToDevice, stream));
     if (geometry) {
         std::vector<int>& off = sc->light_offsets;
         off.assign(L + 1, 0);
@@ -140,7 +197,7 @@ int rb_build_lights(rb_scene* sc, bool geometry, cudaStream_t stream) {
             LightAux init;
             init.bounds[0] = init.bounds[1] = 0xff800000u; // +inf
             init.bounds[2] = init.bounds[3] = 0x007fffffu; // -inf
-            init.status = 0;
+            init.status = init.uv_status = 0;
             RB_CUDA_OK(cudaMemcpyAsync(aux, &init, sizeof(init), cudaMemcpyHostToDevice, stream));
             long long V = 0;
             for (const rb_shape& s : sc->shapes) V = std::max<long long>(V, s.num_vertices);
@@ -155,7 +212,46 @@ int rb_build_lights(rb_scene* sc, bool geometry, cudaStream_t stream) {
         d_pool = (double*)sc->bufs[SS_AREA_POOL].p;
         d_off = (int*)sc->bufs[SS_AREA_OFFSETS].p;
     }
-    k_lt_pmf<<<1, 1, 0, stream>>>(d_lights, L, d_areas, env ? 1 : 0, (int)sc->shapes.size(), env ? (double)sc->dev.env.pdf_norm : 0.0, aux, d_pmf, d_cdf);
+    // emission sampling: every table of every light that samples by its texture, on every call (texels change in place between updates)
+    LightSampling* d_sel = nullptr;
+    std::vector<size_t> off_unused;
+    RB_CUDA_OK(cudaMemsetAsync(&aux->uv_status, 0, sizeof(int), stream));
+    if (host_any(sc->light_sampling)) {
+        std::vector<size_t> off;
+        const size_t n = host_light_sampling_layout(sc->light_sampling, sc->light_emission, sc->lights, sc->shapes, off);
+        const size_t head = (sizeof(LightSampling) * (size_t)L + sizeof(double) - 1) / sizeof(double); // (descriptors, then the data)
+        double* pool;
+        if (scene_table(sc, SS_LIGHT_SAMPLING, head + n, stream, &pool)) return 1;
+        d_sel = (LightSampling*)pool;
+        std::vector<LightSampling> desc(L);
+        const int B = 256;
+        for (int l = 0; l < L; l++) {
+            if (!sc->light_sampling[l]) {
+                desc[l] = LightSampling{nullptr, 0, 0};
+                continue;
+            }
+            const rb_texture& t = sc->light_emission[l];
+            const int w = t.width[0], h = t.height[0], T = sc->shapes[sc->lights[l].shape_id].num_triangles;
+            double* d = pool + head + off[l];
+            desc[l] = LightSampling{d, w, h};
+            const long long C = (long long)w * h;
+            k_ls_cells<<<(unsigned)((C + B - 1) / B), B, 0, stream>>>(t, d);
+            k_ls_rows<<<(h + B - 1) / B, B, 0, stream>>>(w, h, d);
+            k_ls_cols<<<(w + B - 1) / B, B, 0, stream>>>(w, h, d);
+            if (T > 0) k_ls_tris<<<(T + B - 1) / B, B, 0, stream>>>(sc->dev.shapes, sc->lights[l].shape_id, t, d, aux);
+            k_ls_scan<<<1, 32, 0, stream>>>(T, w, h, d);
+        }
+        RB_CUDA_OK(cudaMemcpyAsync(d_sel, desc.data(), sizeof(LightSampling) * (size_t)L, cudaMemcpyHostToDevice, stream));
+    }
+    sc->light_sampling_bytes = 0;
+    if (d_sel) {
+        sc->light_sampling_head = ((sizeof(LightSampling) * (size_t)L + sizeof(double) - 1) / sizeof(double)) * sizeof(double);
+        sc->light_sampling_bytes = sizeof(double) * host_light_sampling_layout(sc->light_sampling, sc->light_emission, sc->lights, sc->shapes, off_unused);
+    }
+    // the light table's last word: the descriptors' address (rb_types.cuh)
+    const unsigned long long word = (unsigned long long)(uintptr_t)d_sel;
+    RB_CUDA_OK(cudaMemcpyAsync(d_table + sc->light_table.size() - 1, &word, sizeof(word), cudaMemcpyHostToDevice, stream));
+    k_lt_pmf<<<1, 1, 0, stream>>>(d_lights, L, d_areas, d_sel, env ? 1 : 0, (int)sc->shapes.size(), env ? (double)sc->dev.env.pdf_norm : 0.0, aux, d_pmf, d_cdf);
     RB_CUDA_OK(cudaGetLastError());
     sc->dev.lights = d_lights;
     sc->dev.light_pmf = d_pmf;
@@ -166,11 +262,14 @@ int rb_build_lights(rb_scene* sc, bool geometry, cudaStream_t stream) {
     return 0;
 }
 
-// 0: the light tables of the last rb_build_lights are valid; 1: their total importance was not positive.  Synchronises the stream.
+// 0: the light tables of the last rb_build_lights are valid; 1: their total importance was not positive; 2: a light's texture coordinates
+// are out of the range of emission sampling.  Synchronises the stream.
 int rb_light_status(const rb_scene* sc, cudaStream_t stream, int* status) {
     *status = 0;
     if (sc->dev.num_lights == 0) return 0;
-    RB_CUDA_OK(cudaMemcpyAsync(status, (const char*)sc->bufs[SS_LIGHT_AUX].p + offsetof(LightAux, status), sizeof(int), cudaMemcpyDeviceToHost, stream));
+    int st[2] = {0, 0};
+    RB_CUDA_OK(cudaMemcpyAsync(st, (const char*)sc->bufs[SS_LIGHT_AUX].p + offsetof(LightAux, status), 2 * sizeof(int), cudaMemcpyDeviceToHost, stream));
     RB_CUDA_OK(cudaStreamSynchronize(stream));
+    *status = st[1] ? 2 : st[0];
     return 0;
 }

@@ -29,6 +29,9 @@ struct LightSampleRec {
     Isect isect;      // (light shape, triangle); environment map: shape_id = -1 and tri_id = bits of dir.z
     V2 uv;            // the 2-D sample used on the triangle; environment map: (dir.x, dir.y) of the sampled direction
     bool unoccluded;  // shadow ray reached the light (nee_ray.tmax >= 0)
+#if RB_LIGHT_TEX_KERNELS
+    bool rejected;    // emission sampling placed the point outside the triangle: no light sample at all (unoccluded is false too)
+#endif
 };
 // The environment-map sample keeps its world direction in the record (the adjoint pass needs exactly the direction the
 // primal pass used; re-sampling from rounded random numbers would not give it).
@@ -73,10 +76,184 @@ RB_D D3 hit_point_d(const rb_shape& s, int tri, D3 o, D3 d) {
     return d3(o.x + d.x * t, o.y + d.y * t, o.z + d.z * t);
 }
 
+// ---- emission sampling (rb_area_light::emission_sampling, DESIGN.md "Emission sampling")
+#if RB_LIGHT_TEX_KERNELS
+#include "rb_light_build.cuh"
+#endif
+// The tables of light l's texture branch, or null when the light samples by area (always null where RB_LIGHT_TEX cannot hold).
+RB_HD const LightSampling* light_sampling(const DevScene& sc, int l) {
+#if RB_LIGHT_TEX_KERNELS
+    const LightSampling* t = light_sampling_table(sc);
+    if (t == nullptr || t[l].data == nullptr || !(t[l].data[0] > 0)) return nullptr;
+    return t + l;
+#else
+    (void)sc;
+    (void)l;
+    return nullptr;
+#endif
+}
+#if RB_LIGHT_TEX_KERNELS // (the kernel sets without emission textures compile none of it: their code stays what it was)
+// THE density of light l's point sampler (per unit area, without the light's selection probability) at the point of triangle `tri`
+// whose texture coordinate, before uv_scale, is `uv`: delta / A_l + (1 - delta) P_t (w_c / M_t) |T_t| / area_t, with c the cell at uv
+// clamped into the triangle's rectangle R_t.  Every estimator that weighs a point of such a light calls it, from the point alone.
+RB_HD double light_point_density(const DevScene& sc, const LightSampling& s, int l, int tri, V2 uv) {
+    const rb_texture& et = light_emission(sc, l);
+    const double* r = s.data + ls_tris(s.w, s.h) + RB_LS_TRI * (size_t)tri;
+    const double X = (double)uv.x * (double)et.uv_scale[0] * s.w - 0.5, Y = (double)uv.y * (double)et.uv_scale[1] * s.h - 0.5;
+    const long long ix = (long long)fmin(fmax(floor(X), r[0]), r[2] - 1), iy = (long long)fmin(fmax(floor(Y), r[1]), r[3] - 1);
+    const long long cx = ix - ls_floor_div(ix, s.w) * s.w, cy = iy - ls_floor_div(iy, s.h) * s.h;
+    const double wc = s.data[ls_cells(s.w, s.h) + (size_t)cy * s.w + (size_t)cx];
+    return RB_LS_DELTA / sc.light_areas[l] + (1 - RB_LS_DELTA) * r[7] * wc;
+}
+// The texture branch: triangle by the CDF of a_t at u1, then a row of R_t by sv and a column within it by su from the summed-area table,
+// each continuous inside its cell, and the barycentrics (b1, b2) of that point in the triangle's cell-space corners.  False: rejected (the
+// point lies outside the triangle, or a degenerate table row).
+RB_HD bool ls_sample_tex(const LightSampling& s, const rb_texture& et, const rb_shape& shape, double u1, double su, double sv, int& tri, double& b1,
+                         double& b2) {
+    const int T = shape.num_triangles, w = s.w, h = s.h;
+    const double *recs = s.data + ls_tris(w, h), *sat = s.data + ls_sat(w, h);
+    int lo = 0, hi = T; // (upper_bound, as cdf_pick)
+    while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (recs[RB_LS_TRI * (size_t)mid + 6] <= u1) lo = mid + 1;
+        else hi = mid;
+    }
+    tri = rb_clampi(lo - 1, 0, T - 1);
+    const double* r = recs + RB_LS_TRI * (size_t)tri;
+    if (!(r[5] > 0)) return false;
+    // (in R_t moved by whole periods so that its corner lies in the first period, as ls_rect_mass does: small prefixes)
+    const long long bx = ls_floor_div((long long)r[0], w) * w, by = ls_floor_div((long long)r[1], h) * h;
+    const long long x0 = (long long)r[0] - bx, y0 = (long long)r[1] - by, x1 = (long long)r[2] - bx, y1 = (long long)r[3] - by;
+    // rows: the mass of [x0, x1) x [y0, y) is strip(y) - strip(y0)
+    auto strip = [&](long long y) { return ls_prefix(sat, w, h, x1, y) - ls_prefix(sat, w, h, x0, y); };
+    const double rbase = strip(y0), ty = sv * (strip(y1) - rbase);
+    long long a = y0, b = y1;
+    while (b - a > 1) {
+        const long long mid = a + (b - a) / 2;
+        if (strip(mid) - rbase <= ty) a = mid;
+        else b = mid;
+    }
+    const long long j = a;
+    const double r0 = strip(j) - rbase, r1 = strip(j + 1) - rbase;
+    if (!(r1 > r0)) return false;
+    // columns of row j: the mass of [x0, x) x [j, j + 1) is col(x) - col(x0)
+    auto col = [&](long long x) { return ls_prefix(sat, w, h, x, j + 1) - ls_prefix(sat, w, h, x, j); };
+    const double cbase = col(x0), tx = su * (col(x1) - cbase);
+    a = x0;
+    b = x1;
+    while (b - a > 1) {
+        const long long mid = a + (b - a) / 2;
+        if (col(mid) - cbase <= tx) a = mid;
+        else b = mid;
+    }
+    const long long i = a;
+    const double c0 = col(i) - cbase, c1 = col(i + 1) - cbase;
+    if (!(c1 > c0)) return false;
+    const double X = (double)(i + bx) + fmin(fmax((tx - c0) / (c1 - c0), 0.0), 1.0), Y = (double)(j + by) + fmin(fmax((ty - r0) / (r1 - r0), 0.0), 1.0);
+    double CX[3], CY[3];
+    ls_tri_corners(shape, tri, et.uv_scale[0], et.uv_scale[1], w, h, CX, CY);
+    const double e1x = CX[1] - CX[0], e1y = CY[1] - CY[0], e2x = CX[2] - CX[0], e2y = CY[2] - CY[0], dx = X - CX[0], dy = Y - CY[0];
+    const double det = e1x * e2y - e1y * e2x;
+    b1 = (dx * e2y - dy * e2x) / det;
+    b2 = (e1x * dy - e1y * dx) / det;
+    return b1 >= 0 && b2 >= 0 && b1 + b2 <= 1;
+}
+// A point on area light l: the triangle and the barycentrics (b1, b2) the shadow ray is built from, the equivalent uniform sample
+// (su', sv') = ((1 - b1)^2, b2 / (1 - b1)) that the record keeps (sample_light_triangle and light_sample_uv reproduce the point from it),
+// the branch (0: by area, 1: by texture) and whether the texture branch rejected the point.  A light without emission sampling takes
+// today's uniform map of (su, sv).
+struct LightPoint {
+    int tri, branch;
+    bool rejected;
+    double b1, b2, su, sv;
+};
+RB_D LightPoint sample_light_point(const DevScene& sc, int l, double tri_sel, double su, double sv) {
+    const rb_shape& shape = sc.shapes[sc.lights[l].shape_id];
+    const double* acdf = sc.area_cdf_pool + sc.area_cdf_offset[l];
+    const LightSampling* s = light_sampling(sc, l);
+    LightPoint p;
+    p.branch = 0;
+    p.rejected = false;
+    if (s == nullptr || tri_sel < RB_LS_DELTA) {
+        p.tri = cdf_pick(acdf, shape.num_triangles, s ? tri_sel / RB_LS_DELTA : tri_sel);
+        double a = sqrt(su);
+        p.b1 = 1.0 - a;
+        p.b2 = a * sv;
+        p.su = su;
+        p.sv = sv;
+        return p;
+    }
+    p.branch = 1;
+    p.rejected = !ls_sample_tex(*s, light_emission(sc, l), shape, (tri_sel - RB_LS_DELTA) / (1 - RB_LS_DELTA), su, sv, p.tri, p.b1, p.b2);
+    if (p.rejected) {
+        p.b1 = p.b2 = p.su = p.sv = 0;
+        return p;
+    }
+    const double a = 1 - p.b1;
+    p.su = a * a;
+    p.sv = a > 0 ? p.b2 / a : 0.0;
+    return p;
+}
+// light_point_density for any area light: 1 / A_l for a light that samples by area.
+RB_HD double light_point_pdf(const DevScene& sc, int l, int tri, V2 uv) {
+    const LightSampling* s = light_sampling(sc, l);
+    return s ? light_point_density(sc, *s, l, tri, uv) : 1.0 / sc.light_areas[l];
+}
+// Test hook rb_light_sample_test, sample i: { branch, triangle, rejected } and { b1, b2, density } of the record sample_light would keep
+// (b1, b2 as sample_light_triangle reproduces them from it); query k: the density at { triangle, u, v } (NaN for a triangle out of range).
+RB_D void light_sample_test_one(const DevScene& sc, int l, const double* samples, int n, int* ints, double* doubles, const float* queries, int m,
+                                 double* query_pdfs, long long i) {
+    const rb_shape& shape = sc.shapes[sc.lights[l].shape_id];
+    if (i < n) {
+        const double* q = samples + 3 * i;
+        const LightPoint p = sample_light_point(sc, l, q[0], q[1], q[2]);
+        ints[3 * i] = p.branch;
+        ints[3 * i + 1] = p.tri;
+        ints[3 * i + 2] = p.rejected ? 1 : 0;
+        double* o = doubles + 3 * i;
+        o[0] = o[1] = o[2] = 0;
+        if (!p.rejected) {
+            const V2 rec = mk2((Real)p.su, (Real)p.sv);
+            const Real a = sqrt(rec.x);
+            o[0] = 1 - a;
+            o[1] = a * rec.y;
+            o[2] = light_point_pdf(sc, l, p.tri, light_sample_uv(shape, p.tri, rec));
+        }
+    }
+    if (i < m) {
+        const float* q = queries + 3 * i;
+        const int tri = (int)q[0];
+        query_pdfs[i] = tri >= 0 && tri < shape.num_triangles ? light_point_pdf(sc, l, tri, mk2(q[1], q[2])) : NAN;
+    }
+}
+// Whether the shadow ray from the double hit point `p_d` to the point (b1, b2) of triangle `tri` reaches it (built in double, then
+// rounded once -- src/scene.cpp:692-741; sample_light's uniform path spells the same steps out, so that the kernels without emission
+// textures compile to the code they had).
+RB_D bool light_point_unoccluded(const DevScene& sc, const rb_shape& shape, int tri, double b1, double b2, D3 p_d) {
+    int idx[3];
+    shape_tri(shape, tri, idx);
+    const float *p0 = shape.vertices + 3 * (size_t)idx[0], *p1 = shape.vertices + 3 * (size_t)idx[1], *p2 = shape.vertices + 3 * (size_t)idx[2];
+    double lx = p0[0] + ((double)p1[0] - p0[0]) * b1 + ((double)p2[0] - p0[0]) * b2;
+    double ly = p0[1] + ((double)p1[1] - p0[1]) * b1 + ((double)p2[1] - p0[1]) * b2;
+    double lz = p0[2] + ((double)p1[2] - p0[2]) * b1 + ((double)p2[2] - p0[2]) * b2;
+    double dx = lx - p_d.x, dy = ly - p_d.y, dz = lz - p_d.z;
+    double len = sqrt(dx * dx + dy * dy + dz * dz);
+    Ray sh;
+    sh.org = mk3((Real)p_d.x, (Real)p_d.y, (Real)p_d.z);
+    sh.dir = len > 0 ? mk3((Real)(dx / len), (Real)(dy / len), (Real)(dz / len)) : zero3();
+    sh.tmin = Real(1e-3);
+    sh.tmax = (Real)((1 - 1e-3f) * len);
+    return !any_hit(sc, sh);
+}
+#endif
+
 // Pick a light, a triangle on it and a point on the triangle; trace the shadow ray (built in double from the double hit
 // point `p_d`, then rounded once -- src/scene.cpp:692-741).
 RB_D void sample_light(const DevScene& sc, D3 p_d, double light_sel, double tri_sel, double su, double sv, LightSampleRec& rec, SurfacePoint& lp) {
     int light_id = cdf_pick(sc.light_cdf, sc.num_lights, light_sel);
+#if RB_LIGHT_TEX_KERNELS
+    rec.rejected = false;
+#endif
     if (RB_ENVMAP(sc) && light_id == sc.num_lights - 1) {
         // environment map: direction by importance sampling, shadow ray to infinity (src/scene.cpp:703-711)
         V3 dir = envmap_sample(sc.env, su, sv);
@@ -92,6 +269,23 @@ RB_D void sample_light(const DevScene& sc, D3 p_d, double light_sel, double tri_
     }
     const DevLight& light = sc.lights[light_id];
     const rb_shape& shape = sc.shapes[light.shape_id];
+#if RB_LIGHT_TEX_KERNELS
+    if (light_sampling(sc, light_id) != nullptr) { // emission sampling: the point from sample_light_point, the record from its equivalent sample
+        const LightPoint q = sample_light_point(sc, light_id, tri_sel, su, sv);
+        rec.isect.shape_id = light.shape_id;
+        rec.isect.tri_id = q.tri;
+        rec.uv = mk2((Real)q.su, (Real)q.sv);
+        if (q.rejected) {
+            rec.rejected = true;
+            rec.unoccluded = false;
+            lp = zero_point();
+            return;
+        }
+        lp = sample_light_triangle(shape, q.tri, rec.uv);
+        rec.unoccluded = light_point_unoccluded(sc, shape, q.tri, q.b1, q.b2, p_d);
+        return;
+    }
+#endif
     const double* acdf = sc.area_cdf_pool + sc.area_cdf_offset[light_id];
     int tri = cdf_pick(acdf, shape.num_triangles, tri_sel);
     rec.isect.shape_id = light.shape_id;
@@ -194,11 +388,23 @@ RB_D V3 vertex_estimate(const DevScene& sc, const rb_material& mat, const Surfac
                 const DevLight& light = sc.lights[lshape.light_id];
                 if (light.two_sided || dot(-wo, lp.shading_frame.n) > 0) {
                     G = fabs(dot(wo, lp.geom_normal)) / dist_sq;
+#if !RB_LIGHT_TEX_KERNELS
                     pdf_nee = (Real)(sc.light_pmf[lshape.light_id] / sc.light_areas[lshape.light_id]);
+#endif
                     Le = mk3(light.intensity[0], light.intensity[1], light.intensity[2]);
                     // (an emission texture: at the sample's uv, unfiltered like the environment map's lookups)
                     const rb_texture& et = light_emission(sc, lshape.light_id);
+#if RB_LIGHT_TEX_KERNELS
+                    const LightSampling* lsm = light_sampling(sc, lshape.light_id);
+                    if (RB_LIGHT_TEX(et)) {
+                        const V2 luv = light_sample_uv(lshape, ls.isect.tri_id, ls.uv);
+                        Le = Le * light_tex_eval(et, luv, zero2(), zero2());
+                        if (lsm) pdf_nee = (Real)(sc.light_pmf[lshape.light_id] * light_point_density(sc, *lsm, lshape.light_id, ls.isect.tri_id, luv));
+                    }
+                    if (!lsm) pdf_nee = (Real)(sc.light_pmf[lshape.light_id] / sc.light_areas[lshape.light_id]);
+#else
                     if (RB_LIGHT_TEX(et)) Le = Le * light_tex_eval(et, light_sample_uv(lshape, ls.isect.tri_id, ls.uv), zero2(), zero2());
+#endif
                     on = true;
                 }
             }
@@ -238,7 +444,13 @@ RB_D V3 vertex_estimate(const DevScene& sc, const rb_material& mat, const Surfac
                     const DevLight& light = sc.lights[bshape.light_id];
                     if (light.two_sided || dot(-wo, bp.shading_frame.n) > 0) {
                         Real G = fabs(dot(wo, bp.geom_normal)) / dist_sq;
+#if RB_LIGHT_TEX_KERNELS
+                        const LightSampling* lsm = light_sampling(sc, bshape.light_id);
+                        Real pdf_nee = (Real)(lsm ? sc.light_pmf[bshape.light_id] * light_point_density(sc, *lsm, bshape.light_id, bis.tri_id, bp.uv)
+                                                  : sc.light_pmf[bshape.light_id] * (1.0 / sc.light_areas[bshape.light_id])) / G;
+#else
                         Real pdf_nee = (Real)(sc.light_pmf[bshape.light_id] * (1.0 / sc.light_areas[bshape.light_id])) / G;
+#endif
                         V3 Le = mk3(light.intensity[0], light.intensity[1], light.intensity[2]);
                         const rb_texture& et = light_emission(sc, bshape.light_id);
                         if (RB_LIGHT_TEX(et)) Le = Le * light_tex_eval(et, bp.uv, zero2(), zero2());
@@ -424,8 +636,12 @@ RB_D VertexAdjoint d_vertex(const DevScene& sc, const DevDScene& ds, const Verte
                         E_l = light_tex_eval(et, luv, zero2(), zero2());
                         Le = Le * E_l;
                     }
-#endif
+                    const LightSampling* lsm = light_sampling(sc, lshape.light_id);
+                    pdf_nee = (Real)(lsm ? sc.light_pmf[lshape.light_id] * light_point_density(sc, *lsm, lshape.light_id, lis.tri_id, luv)
+                                         : sc.light_pmf[lshape.light_id] * (1.0 / sc.light_areas[lshape.light_id]));
+#else
                     pdf_nee = (Real)(sc.light_pmf[lshape.light_id] * (1.0 / sc.light_areas[lshape.light_id]));
+#endif
                     ok = true;
                 }
             }
@@ -529,7 +745,13 @@ RB_D VertexAdjoint d_vertex(const DevScene& sc, const DevDScene& ds, const Verte
                             Le = Le * E_b;
                         }
 #endif
+#if RB_LIGHT_TEX_KERNELS
+                        const LightSampling* lsm = light_sampling(sc, bshape.light_id);
+                        Real pdf_nee = (Real)(lsm ? sc.light_pmf[bshape.light_id] * light_point_density(sc, *lsm, bshape.light_id, bis.tri_id, bp.uv)
+                                                  : sc.light_pmf[bshape.light_id] * (1.0 / sc.light_areas[bshape.light_id])) / G;
+#else
                         Real pdf_nee = (Real)(sc.light_pmf[bshape.light_id] * (1.0 / sc.light_areas[bshape.light_id])) / G;
+#endif
                         Real wgt = mis_power2(pdf_nee, pdf_b) / pdf_b;
                         out.d_thr += d_contrib * (wgt * f * Le);
                         d_f += wgt * (d_scatter * Le);

@@ -30,7 +30,7 @@ struct EventPool {
 // frees it in stream order and allocates a new one, so an update that rebuilds a table replaces it instead of adding to it.
 enum SceneSlot {
     SS_SHAPES, SS_MATERIALS, SS_BVH_NODES, SS_BVH_TRIS, SS_LIGHTS, SS_LIGHT_PMF, SS_LIGHT_CDF, SS_LIGHT_AREAS, SS_AREA_POOL, SS_AREA_OFFSETS,
-    SS_LIGHT_AUX, SS_EDGES, SS_PRIM_PMF, SS_PRIM_CDF, SS_EDGE_NODES, SS_COUNT
+    SS_LIGHT_AUX, SS_EDGES, SS_PRIM_PMF, SS_PRIM_CDF, SS_EDGE_NODES, SS_LIGHT_SAMPLING, SS_COUNT
 };
 struct SceneBuffer {
     void* p = nullptr;
@@ -49,7 +49,9 @@ struct rb_scene {
     std::vector<rb_material> materials;
     std::vector<DevLight> lights;
     std::vector<rb_texture> light_emission;      // per area light: its emission texture (num_levels == 0: none)
-    std::vector<unsigned long long> light_table; // what SS_LIGHTS holds: the DevLights, then the emission textures (light_emission)
+    std::vector<unsigned long long> light_table; // what SS_LIGHTS holds: the DevLights, the emission textures (light_emission), the sampling word
+    std::vector<int> light_sampling;             // per area light: 1 when it samples by its emission texture (host_light_sampling)
+    size_t light_sampling_head = 0, light_sampling_bytes = 0; // SS_LIGHT_SAMPLING: bytes of descriptors before the data, bytes of data (0: none)
     std::vector<int> light_offsets; // [lights + 1]: first entry of every light in the area-CDF pool, then the pool size
     int max_generic_texture_dimension = 0;
     int has_envmap = 0;

@@ -87,6 +87,8 @@ inline const char* host_check_scene_desc(const rb_scene_desc& desc) {
     for (int l = 0; l < desc.num_lights; l++) {
         if (desc.lights[l].shape_id < 0 || desc.lights[l].shape_id >= desc.num_shapes) return "rb_scene_create: area light refers to an invalid shape";
         if (const char* err = host_check_emission(desc.lights[l].emission)) return err;
+        if (desc.lights[l].emission_sampling != RB_EMISSION_SAMPLE_AREA && desc.lights[l].emission_sampling != RB_EMISSION_SAMPLE_TEXTURE)
+            return "rb_scene_create: a light's emission_sampling must be RB_EMISSION_SAMPLE_AREA (0) or RB_EMISSION_SAMPLE_TEXTURE (1)";
     }
     for (int s = 0; s < desc.num_shapes; s++) {
         const rb_shape& sh = desc.shapes[s];
@@ -112,6 +114,61 @@ inline std::vector<rb_texture> host_light_emission(const rb_scene_desc& desc) {
     std::vector<rb_texture> out;
     for (int l = 0; l < desc.num_lights; l++) out.push_back(desc.lights[l].emission);
     return out;
+}
+// Per area light: 1 when it samples by its emission texture (RB_EMISSION_SAMPLE_TEXTURE and a texture that is not constant), else 0.
+inline std::vector<int> host_light_sampling(const rb_scene_desc& desc) {
+    std::vector<int> out;
+    for (int l = 0; l < desc.num_lights; l++) {
+        const rb_texture& t = desc.lights[l].emission;
+        out.push_back(desc.lights[l].emission_sampling == RB_EMISSION_SAMPLE_TEXTURE && t.num_levels > 0 && !(t.width[0] == 0 && t.height[0] == 0) ? 1 : 0);
+    }
+    return out;
+}
+inline bool host_any(const std::vector<int>& v) {
+    for (int x : v)
+        if (x) return true;
+    return false;
+}
+// Layout of the emission-sampling data: per light its offset into the pool (doubles) and its level-0 size; returns the pool size.
+inline size_t host_light_sampling_layout(const std::vector<int>& on, const std::vector<rb_texture>& emission, const std::vector<DevLight>& lights,
+                                         const std::vector<rb_shape>& shapes, std::vector<size_t>& offsets) {
+    size_t n = 0;
+    offsets.assign(on.size(), 0);
+    for (size_t l = 0; l < on.size(); l++) {
+        offsets[l] = n;
+        if (on[l]) n += ls_size(emission[l].width[0], emission[l].height[0], shapes[lights[l].shape_id].num_triangles);
+    }
+    return n;
+}
+const char* const RB_LS_UV_ERROR =
+    "rb_scene_create: emission sampling needs the scaled texture coordinates of a light (uv * uv_scale * level-0 size) to be finite and below 2^24 cells in magnitude";
+// The emission-sampling tables with the steps of rb_light_build.cuh in serial loops (`shapes` and the textures hold host pointers): fills
+// `pool` and, per light, S[l] (0 for a light that samples by area).  Returns false with `err` set when a light's texture coordinates are out
+// of range.
+inline bool host_build_light_sampling(const std::vector<int>& on, const std::vector<rb_texture>& emission, const std::vector<DevLight>& lights,
+                                      const std::vector<rb_shape>& shapes, const std::vector<size_t>& offsets, std::vector<double>& pool,
+                                      std::vector<double>& S, std::string& err) {
+    S.assign(on.size(), 0.0);
+    for (size_t l = 0; l < on.size(); l++) {
+        if (!on[l]) continue;
+        const rb_texture& t = emission[l];
+        const int w = t.width[0], h = t.height[0];
+        const rb_shape& sh = shapes[lights[l].shape_id];
+        double* d = pool.data() + offsets[l];
+        double *cells = d + ls_cells(w, h), *sat = d + ls_sat(w, h), *recs = d + ls_tris(w, h);
+        for (int j = 0; j < h; j++)
+            for (int i = 0; i < w; i++) cells[(size_t)j * w + i] = ls_cell_weight(t.texels[0], t.channels, w, h, i, j);
+        for (int j = 0; j < h; j++) ls_sat_row(cells, sat, w, j);
+        for (int i = 0; i < w; i++) ls_sat_col(sat, w, h, i);
+        for (int k = 0; k < sh.num_triangles; k++)
+            if (!ls_tri_record(sh, k, t.uv_scale[0], t.uv_scale[1], w, h, sat, recs + RB_LS_TRI * (size_t)k)) {
+                err = RB_LS_UV_ERROR;
+                return false;
+            }
+        d[0] = S[l] = ls_scan(recs, sh.num_triangles);
+        d[1] = 0;
+    }
+    return true;
 }
 inline int host_max_generic_texture_dimension(const rb_scene_desc& desc) {
     int n = 0;
@@ -173,8 +230,9 @@ inline double host_bsphere_radius(const std::vector<HostMesh>& meshes) {
 }
 // `has_env` appends the environment map as the last light (src/scene.cpp:197-253).  The steps are those of rb_light_build.cuh, which
 // rb_light_build.cu runs on the device.
+// `sel`: per light, S of its emission sampling (ls_selection_area), or null.
 inline bool host_build_lights(const std::vector<DevLight>& lights, const std::vector<HostMesh>& meshes, HostLightTables& out, std::string& err,
-                              bool has_env = false, double env_pdf_norm = 0, double bsphere_radius = 0) {
+                              bool has_env = false, double env_pdf_norm = 0, double bsphere_radius = 0, const std::vector<double>* sel = nullptr) {
     int L = (int)lights.size();
     out.pmf.assign(L, 0);
     out.cdf.assign(L, 0);
@@ -189,7 +247,7 @@ inline bool host_build_lights(const std::vector<DevLight>& lights, const std::ve
         for (int t = 0; t < T; t++) a[t] = lt_triangle_area(m.vertices.data(), &m.indices[3 * (size_t)t]);
         out.pool.resize(out.pool.size() + T);
         out.areas[l] = lt_sum_and_scan(a.data(), T, out.pool.data() + out.offsets[l]);
-        out.pmf[l] = lt_light_weight(lights[l], out.areas[l]);
+        out.pmf[l] = lt_light_weight(lights[l], sel ? ls_selection_area(out.areas[l], (*sel)[l]) : out.areas[l]);
     }
     if (has_env) {
         out.pmf.push_back(lt_env_weight(bsphere_radius, env_pdf_norm));

@@ -338,7 +338,14 @@ RB_D int sample_edge_gather(const EdgeCtx& c, const Ray& nee, const Isect& lis, 
     Real tau = dot(lp.position - nee.org, nn) / dot(omega, nn);
     Real jac = length(tau * ((v1 - v0) - omega * (dot(v1 - v0, nn) / dot(omega, nn))));
     const rb_shape& lshape = sc.shapes[lis.shape_id];
+#if RB_LIGHT_TEX_KERNELS
+    // (emission sampling: the density at the light point, whose record sample lp.uv gives its texture coordinate)
+    const LightSampling* lsm = light_sampling(sc, lshape.light_id);
+    Real pdf_nee = (Real)(lsm ? sc.light_pmf[lshape.light_id] * light_point_density(sc, *lsm, lshape.light_id, lis.tri_id, light_sample_uv(lshape, lis.tri_id, lp.uv))
+                              : sc.light_pmf[lshape.light_id] / sc.light_areas[lshape.light_id]);
+#else
     Real pdf_nee = (Real)(sc.light_pmf[lshape.light_id] / sc.light_areas[lshape.light_id]);
+#endif
     if (pmf <= 0 || jac <= 0 || pdf_nee <= 0) return -1;
     sample_weight = 1 / (2 * expand * pmf * jac * pdf_nee);
     V3 v0_p = v0 - ip;
@@ -511,6 +518,9 @@ RB_D bool secondary_edge_pick(const DevScene& sc, const VertexRec& cur, Sampler&
         int edge_id = sample_edge_hier(ps.c, ps.edge_sel, ps.resample, edge_weight);
         return pick_finish_hier(sc, ps, edge_id, edge_weight, pk);
     }
+#if RB_LIGHT_TEX_KERNELS
+    if (cur.light.rejected) return false; // (emission sampling rejected the light point: no shadow ray to gather along)
+#endif
     Real edge_weight = 0;
     V3 sample_p = zero3(), mwt = zero3();
     int edge_id = sample_edge_gather(ps.c, nee, cur.light.isect, lp, ps.resample, edge_weight, sample_p, mwt);

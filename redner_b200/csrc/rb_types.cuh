@@ -208,6 +208,20 @@ inline std::vector<unsigned long long> light_table_words(const T* head, const rb
     }
     return w;
 }
+// Emission sampling (rb_area_light::emission_sampling, DESIGN.md "Emission sampling").  The scene's light table ends with one more 8-byte
+// word after the emission textures: 0, or the address of L LightSampling descriptors, when some light samples by its texture.  A light
+// whose descriptor has data == nullptr, or whose S = data[0] is 0, samples by area.  data points at { S, 0 }, the w x h cell weights, their
+// w x h summed-area table and 8 doubles per triangle (ls_cells / ls_sat / ls_tris, rb_light_build.cuh).  The word is not part of
+// RB_TABLE_LIGHTS, so that table is what it was for every scene.
+struct LightSampling {
+    const double* data;
+    int w, h;
+};
+RB_HD size_t light_sampling_word(int num_area_lights) { return light_table_offset((size_t)num_area_lights * sizeof(DevLight)) + (size_t)num_area_lights * sizeof(rb_texture); }
+RB_HD const LightSampling* light_sampling_table(const DevScene& sc) {
+    return *(const LightSampling* const*)((const char*)sc.lights + light_sampling_word(num_area_lights(sc)));
+}
+
 // True when some light has an emission texture (RB_LIGHT_TEX), i.e. when only the general and deterministic kernels compute what the
 // scene asks for.
 inline bool lights_use_emission(const std::vector<rb_texture>& emission) {

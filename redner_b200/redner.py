@@ -253,8 +253,9 @@ class DMaterial:  # src/redner.cpp:153-158
 
 
 class AreaLight:  # src/redner.cpp:160-164, src/area_light.h:8-36
-    def __init__(self, shape_id, intensity, two_sided, directly_visible, emission=None):
-        """`emission` (redner_b200 extension): a Texture1 or Texture3, the light's emission texture (rb_area_light::emission), or None."""
+    def __init__(self, shape_id, intensity, two_sided, directly_visible, emission=None, emission_sampling=0):
+        """`emission` (redner_b200 extension): a Texture1 or Texture3, the light's emission texture (rb_area_light::emission), or None.
+        `emission_sampling` (redner_b200 extension): rb_emission_sampling, 0 (by area) or 1 (by the emission texture)."""
         a = L.rb_area_light()
         a.shape_id = int(shape_id)
         a.intensity[:] = _read_floats(intensity, 3)
@@ -262,6 +263,7 @@ class AreaLight:  # src/redner.cpp:160-164, src/area_light.h:8-36
         a.directly_visible = int(bool(directly_visible))
         if emission is not None:
             a.emission = emission._c
+        a.emission_sampling = int(emission_sampling)
         self._c = a
 
 
@@ -427,6 +429,34 @@ class Scene:  # src/redner.cpp:62-73, src/scene.cpp:63-307
         if self._lib.rb_scene_trace_rays(self._handle, C.c_void_p(rays.data_ptr()), n, flags, C.c_void_p(ids.data_ptr()), C.c_void_p(t.data_ptr())) != 0:
             raise RuntimeError("redner.Scene.trace_rays: " + L.last_error(self._lib))
         return ids, t
+
+    def light_sample_test(self, light, samples, queries=None):
+        """The point-on-light sampler of area light `light` and its density (rb_light_sample_test): test hook.  `samples` is an [N, 3]
+        float64 tensor (tri_sel, su, sv) on the scene's device, `queries` None or an [M, 3] float32 tensor (triangle, u, v).  Returns
+        ([N, 3] int32 (branch, triangle, rejected), [N, 3] float64 (b1, b2, density), [M] float64 densities or None)."""
+        import torch
+        samples = samples.to(torch.float64).contiguous()
+        if samples.dim() != 2 or samples.shape[1] != 3:
+            raise ValueError("redner.Scene.light_sample_test: samples must have shape [N, 3]")
+        n, dev = samples.shape[0], samples.device
+        ints = torch.empty((n, 3), dtype=torch.int32, device=dev)
+        doubles = torch.empty((n, 3), dtype=torch.float64, device=dev)
+        m, pdfs = 0, None
+        if queries is not None:
+            queries = queries.to(device=dev, dtype=torch.float32).contiguous()
+            if queries.dim() != 2 or queries.shape[1] != 3:
+                raise ValueError("redner.Scene.light_sample_test: queries must have shape [M, 3]")
+            m = queries.shape[0]
+            pdfs = torch.empty(m, dtype=torch.float64, device=dev)
+        stream = 0
+        if samples.is_cuda:
+            torch.cuda.set_device(dev)
+            stream = torch.cuda.current_stream(dev).cuda_stream
+        ptr = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None  # noqa: E731
+        if self._lib.rb_light_sample_test(self._handle, int(light), ptr(samples), n, ptr(ints), ptr(doubles), ptr(queries), m, ptr(pdfs),
+                                          C.c_void_p(stream or 0)) != 0:
+            raise RuntimeError("redner.Scene.light_sample_test: " + L.last_error(self._lib))
+        return ints, doubles, pdfs
 
     def last_stats(self):
         n = C.c_int(0)

@@ -24,7 +24,10 @@ struct rb_scene {
     std::vector<rb_material> materials;
     std::vector<DevLight> lights;
     std::vector<rb_texture> light_emission;      // per area light (num_levels == 0: none)
-    std::vector<unsigned long long> light_table; // what the kernels read at dev.lights: the DevLights, then light_emission
+    std::vector<unsigned long long> light_table; // what the kernels read at dev.lights: the DevLights, then light_emission, then the sampling word
+    std::vector<int> light_sampling;             // per area light: 1 when it samples by its emission texture
+    std::vector<double> ls_pool;                 // the emission-sampling data (RB_TABLE_LIGHT_SAMPLING)
+    std::vector<LightSampling> ls_desc;          // per area light: its descriptor (what the sampling word points at)
     HostLightTables lt;
     HostEdgeTables et;
     HostEdgeTree tree;
@@ -102,6 +105,8 @@ static int emu_build(rb_scene* sc, const rb_scene_desc* desc) {
     sc->lights = host_area_lights(*desc);
     sc->light_emission = host_light_emission(*desc);
     sc->light_table = light_table_words(sc->lights.data(), sc->light_emission.data(), (int)sc->lights.size());
+    sc->light_table.push_back(0); // (the emission-sampling word, rb_types.cuh)
+    sc->light_sampling = host_light_sampling(*desc);
     sc->max_generic = host_max_generic_texture_dimension(*desc);
     d.edge_root_cs = d.edge_root_ncs = RB_EDGE_EMPTY;
     d.shapes = sc->shapes.data();
@@ -154,8 +159,23 @@ static int emu_build(rb_scene* sc, const rb_scene_desc* desc) {
     }
     host_setup_envmap(desc->envmap, d);
     d.num_lights = (int)sc->lights.size() + (d.has_envmap ? 1 : 0);
+    sc->ls_pool.clear();
+    sc->ls_desc.clear();
     if (d.num_lights > 0) {
-        if (!host_build_lights(sc->lights, meshes, sc->lt, g_err, d.has_envmap != 0, d.has_envmap ? desc->envmap->pdf_norm : 0.0, host_bsphere_radius(meshes))) return 1;
+        std::vector<double> S;
+        if (host_any(sc->light_sampling)) {
+            std::vector<size_t> off;
+            sc->ls_pool.assign(host_light_sampling_layout(sc->light_sampling, sc->light_emission, sc->lights, sc->shapes, off), 0.0);
+            if (!host_build_light_sampling(sc->light_sampling, sc->light_emission, sc->lights, sc->shapes, off, sc->ls_pool, S, g_err)) return 1;
+            for (size_t l = 0; l < sc->lights.size(); l++) {
+                const rb_texture& t = sc->light_emission[l];
+                sc->ls_desc.push_back(sc->light_sampling[l] ? LightSampling{sc->ls_pool.data() + off[l], t.width[0], t.height[0]} : LightSampling{nullptr, 0, 0});
+            }
+            sc->light_table.back() = (unsigned long long)(uintptr_t)sc->ls_desc.data();
+        }
+        if (!host_build_lights(sc->lights, meshes, sc->lt, g_err, d.has_envmap != 0, d.has_envmap ? desc->envmap->pdf_norm : 0.0, host_bsphere_radius(meshes),
+                               S.empty() ? nullptr : &S))
+            return 1;
         d.lights = (const DevLight*)sc->light_table.data();
         d.light_pmf = sc->lt.pmf.data();
         d.light_cdf = sc->lt.cdf.data();
@@ -235,7 +255,8 @@ extern "C" int rb_scene_table(const rb_scene* sc, int which, void* out, size_t b
         case RB_TABLE_AREA_CDF_OFFSETS: src = sc->lt.offsets.data(); n = lights ? sizeof(int) * sc->lt.offsets.size() : 0; break;
         case RB_TABLE_PRIMARY_EDGE_PMF: src = sc->et.prim_pmf.data(); n = prim ? sizeof(double) * (size_t)d.num_edges : 0; break;
         case RB_TABLE_PRIMARY_EDGE_CDF: src = sc->et.prim_cdf.data(); n = prim ? sizeof(double) * (size_t)d.num_edges : 0; break;
-        case RB_TABLE_LIGHTS: src = sc->light_table.data(); n = sc->lights.empty() ? 0 : sizeof(unsigned long long) * sc->light_table.size(); break;
+        case RB_TABLE_LIGHTS: src = sc->light_table.data(); n = sc->lights.empty() ? 0 : sizeof(unsigned long long) * (sc->light_table.size() - 1); break;
+        case RB_TABLE_LIGHT_SAMPLING: src = sc->ls_pool.data(); n = lights ? sizeof(double) * sc->ls_pool.size() : 0; break;
         default: g_err = "rb_scene_table: unknown table"; return 1;
     }
     if (size) *size = n;
@@ -372,6 +393,28 @@ extern "C" int rb_envmap_test(const rb_envmap* env, const rb_texture* d_values, 
         sample_dirs[3 * (size_t)i + 2] = d.z;
     }
     return 0;
+}
+// The point-on-light sampler and its density through the same functions as the library's hook, one sample after another.
+extern "C" int rb_light_sample_test(const rb_scene* sc, int light, const double* samples, int n, int* ints, double* doubles, const float* queries, int m,
+                                    double* query_pdfs, void*) {
+    const char* err = nullptr;
+    if (sc == nullptr) err = "null scene";
+    else if (sc->incomplete) err = "the scene's last update failed";
+    else if (light < 0 || light >= (int)sc->lights.size()) err = "light out of range";
+    else if (n < 0 || m < 0) err = "negative number of samples or queries";
+    else if ((n > 0 && (samples == nullptr || ints == nullptr || doubles == nullptr)) || (m > 0 && (queries == nullptr || query_pdfs == nullptr)))
+        err = "null buffer";
+    if (err != nullptr) {
+        g_err = std::string("rb_light_sample_test: ") + err;
+        return 1;
+    }
+#if RB_LIGHT_TEX_KERNELS
+    for (long long i = 0; i < std::max(n, m); i++) light_sample_test_one(sc->dev, light, samples, n, ints, doubles, queries, m, query_pdfs, i);
+    return 0;
+#else
+    g_err = "rb_light_sample_test: this build has no emission textures";
+    return 1;
+#endif
 }
 extern "C" int rb_scene_edge_list(const rb_scene* sc, int* num_edges, int* edges_out, size_t edges_bytes) {
     if (num_edges) *num_edges = sc->dev.num_edges;
