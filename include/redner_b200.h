@@ -433,6 +433,36 @@ int rb_envmap_test(const rb_envmap* env, const rb_texture* d_values, float* d_w2
 int rb_light_sample_test(const rb_scene* scene, int light, const double* samples, int n, int* ints, double* doubles, const float* queries, int m,
                          double* query_pdfs, void* stream);
 
+/* Test hook: n camera queries of one kind (`op`), one per thread, through the camera functions the render kernels call (rb_camera.cuh,
+ * rb_render.cuh), on the camera of a built scene (rb_scene_set_camera re-targets it).  in: [n, 64] doubles, out: [n, 64] doubles, one row per
+ * query; acc: NULL, or [cam_acc_count, n] floats (cam_acc_count: 58, 60 with a lens), the camera-gradient accumulator with query i's column
+ * at acc + i (stride n), which the adjoint ops add to.  lu below is concentric_disc(u1, u2).  Rows (indices):
+ *   RB_CAMTEST_CAMERA      out: c2w 0-15, w2c 16-31, intr_inv 32-40, intr 41-49, distortion 50-57, lens_radius 58, focus_distance 59,
+ *                          clip_near 60, cam_acc_count 61 (the DevCamera the kernels see)
+ *   RB_CAMTEST_RAY         in: sx, sy, u1, u2.  out: cam_sample_primary org 0-2, dir 3-5 (double); cam_primary_ray org 6-8, dir 9-11,
+ *                          org_dx 12-14, org_dy 15-17, dir_dx 18-20, dir_dy 21-23 (float); lu 24-25
+ *   RB_CAMTEST_D_RAY       in: sx, sy, u1, u2, d_org 4-6, d_dir 7-9, want d_screen 10, d(org_dx, org_dy, dir_dx, dir_dy) 11-22, with the
+ *                          differential 23.  d_cam_sample_primary at ((float)sx, (float)sy) or, with the differential, the adjoint of
+ *                          cam_primary_ray as bwd_sweep forms it (d_cam_primary_ray_diff, then d_cam_sample_primary of the three rays); out:
+ *                          d_screen 0-1
+ *   RB_CAMTEST_PROJECT     in: p0 0-2, p1 3-5, u1 6, u2 7.  out: cam_project_d (cam_project_lens_d with a lens) visible 0, q0 1-2, q1 3-4;
+ *                          cam_project of the float ends visible 5, q0 6-7, q1 8-9
+ *   RB_CAMTEST_D_PROJECT   in: p0 0-2, p1 3-5 (rounded to float), u1 6, u2 7, d_q0 8-9, d_q1 10-11.  d_cam_project (d_cam_project_lens with a
+ *                          lens); out: d_p0 0-2, d_p1 3-5
+ *   RB_CAMTEST_DISTORT     in: pos 0-1, d_out 2-3.  out: cam_distort 0-1 with Jacobian rows d(x)/d(pos) 2-3, d(y)/d(pos) 4-5;
+ *                          cam_inverse_distort 6-7; d_pos of d_cam_distort 8-9 and of d_cam_inverse_distort 10-11; their parameter
+ *                          gradients 12-19 and 20-27
+ *   RB_CAMTEST_FINISH      in: the 60 reduced accumulator doubles.  out: finish_camera's d(position) 0-2, d(look) 3-5, d(up) 6-8 (look-at
+ *                          cameras), d(cam_to_world) 9-24 (the others), d(intrinsic_mat_inv) 25-33, d(intrinsic_mat) 34-42, d(distortion)
+ *                          43-50, d(lens) 51-52
+ * Every buffer is memory of the scene's device; an unknown op, a negative count and an adjoint op without `acc` are refused, as is the
+ * double-precision build.  Runs on `stream` and synchronises it. */
+enum {
+    RB_CAMTEST_CAMERA = 0, RB_CAMTEST_RAY = 1, RB_CAMTEST_D_RAY = 2, RB_CAMTEST_PROJECT = 3, RB_CAMTEST_D_PROJECT = 4, RB_CAMTEST_DISTORT = 5,
+    RB_CAMTEST_FINISH = 6
+};
+int rb_camera_test(const rb_scene* scene, int op, const double* in, int n, double* out, float* acc, void* stream);
+
 const char* rb_last_error(void);
 const char* rb_version(void);
 

@@ -39,8 +39,8 @@ RB_HD D2 cam_distort_impl(const DevCamera& cam, D2 pos, D2* dx_dpos, D2* dy_dpos
     double xx = x * rr + 2 * p0 * x * y + p1 * (r2 + 2 * x * x), yy = y * rr + p0 * (r2 + 2 * y * y) + 2 * p1 * x * y;
     if (dx_dpos != nullptr && dy_dpos != nullptr) {
         D2 dx = d2(2, 0), dy = d2(0, 2); // d(x)/d(pos), d(y)/d(pos)
-        D2 dr = d2((dx.x * x + dy.x * y) / r, (dx.y * x + dy.y * y) / r);
-        D2 dr2 = d2(2 * r * dr.x, 2 * r * dr.y), dr4 = d2(2 * r2 * dr2.x, 2 * r2 * dr2.y);
+        // d(r2) = 2 (x dx + y dy), formed without dividing by r: finite at the centre, where r = 0 (the reference's d(r) / r is NaN there)
+        D2 dr2 = d2(2 * (dx.x * x + dy.x * y), 2 * (dx.y * x + dy.y * y)), dr4 = d2(2 * r2 * dr2.x, 2 * r2 * dr2.y);
         D2 dr6 = d2(r4 * dr2.x + dr4.x * r2, r4 * dr2.y + dr4.y * r2);
         D2 dnum = d2(k[0] * dr2.x + k[1] * dr4.x + k[2] * dr6.x, k[0] * dr2.y + k[1] * dr4.y + k[2] * dr6.y);
         D2 dden = d2(k[3] * dr2.x + k[4] * dr4.x + k[5] * dr6.x, k[3] * dr2.y + k[4] * dr4.y + k[5] * dr6.y);
@@ -87,9 +87,8 @@ RB_HD void d_cam_distort_impl(const DevCamera& cam, D2 pos, D2 d_out, double* d_
     d_r4 += d_r6 * r2;
     d_r2 += d_r6 * r2; // (r2 where r4 belongs: as in the reference :160)
     d_r2 += 2 * d_r4 * r2;
-    double d_r = 2 * d_r2 * r;
-    d_x += d_r * x / r;
-    d_y += d_r * y / r;
+    d_x += 2 * d_r2 * x; // (d(r2)/dx = 2 x, without the reference's division by r, which is NaN at the centre)
+    d_y += 2 * d_r2 * y;
     d_pos.x += d_x * 2;
     d_pos.y += d_y * 2;
     if (d_params != nullptr) {
@@ -427,7 +426,9 @@ RB_D void d_cam_sample_primary_any(const DevCamera& cam, Real sx_, Real sy_, con
                 Real d_cp = d_dir.x * (-st), d_sp = d_dir.y * (-st), d_st = d_dir.x * (-cp) + d_dir.y * (-sp), d_ct = d_dir.z;
                 Real d_phi = d_cp * (-sp) + d_sp * cp, d_theta = d_ct * (-st) + d_st * ct;
                 Real d_r = d_theta * (Real(RB_PI) / 2);
-                Real d_x = d_phi * (-y / (x * x + y * y)) + d_r * (x / r), d_y = d_phi * (x / (x * x + y * y)) + d_r * (y / r);
+                // at the centre phi is atan2(0, 0) = 0 and d_phi / r tends to -(pi / 2) d_dir.y: the limit of the two quotients below
+                Real d_x = r > 0 ? d_phi * (-y / (x * x + y * y)) + d_r * (x / r) : d_r;
+                Real d_y = r > 0 ? d_phi * (x / (x * x + y * y)) + d_r * (y / r) : -(Real(RB_PI) / 2) * d_dir.y;
                 d_screen->x += 2 * d_x;
                 d_screen->y += 2 * d_y;
             } else {
@@ -504,6 +505,20 @@ RB_D void d_cam_sample_primary(const DevCamera& cam, Real sx, Real sy, const DRa
     acc.add_c2w(d_C);
 }
 
+// Adjoint of cam_primary_ray's ray differential, which is psx (ray(sx + delta, sy) - ray(sx, sy)) / delta and likewise in y, psx = 0.5 / width,
+// psy = 0.5 / height: d_prd becomes the adjoints of the two offset rays (d_ray_dx at (sx + delta, sy), d_ray_dy at (sx, sy + delta)) and a
+// term added to the centre ray's d_ray.  Each of the three then goes through d_cam_sample_primary.
+RB_D void d_cam_primary_ray_diff(const DevCamera& cam, const RayDiff& d_prd, DRay& d_ray, DRay& d_ray_dx, DRay& d_ray_dy) {
+    const Real delta = Real(1e-3);
+    Real psx = Real(0.5) / cam.width, psy = Real(0.5) / cam.height;
+    d_ray_dx.org = d_prd.org_dx * (psx / delta);
+    d_ray_dx.dir = d_prd.dir_dx * (psx / delta);
+    d_ray_dy.org = d_prd.org_dy * (psy / delta);
+    d_ray_dy.dir = d_prd.dir_dy * (psy / delta);
+    d_ray.org += (d_prd.org_dx * (-psx) + d_prd.org_dy * (-psy)) / delta;
+    d_ray.dir += (d_prd.dir_dx * (-psx) + d_prd.dir_dy * (-psy)) / delta;
+}
+
 // ---- screen projection of a world-space segment (primary edge sampling) ----
 RB_HD V2 cam_to_screen_undistorted(const DevCamera& cam, V3 pt);
 RB_HD V2 cam_to_screen(const DevCamera& cam, V3 pt) {
@@ -564,19 +579,29 @@ RB_D void d_cam_to_screen_any(const DevCamera& cam, V3 pt, Real dx, Real dy, Cam
         dy = (Real)d_q.y;
     }
     if (cam.type == RB_CAMERA_FISHEYE) { // src/camera.h:669-697
+        // On the unit sphere the map is s = 1/2 - G(theta) (d.x, d.y) / pi with G = theta / sin(theta), theta = atan2(rho, d.z) and
+        // rho = sqrt(d.x^2 + d.y^2) = sin(theta): smooth at the axis.  Any extension off the sphere gives the same d_pt once
+        // d_normalize drops the radial part, so G is differentiated as a function of d.z alone: G'(z) = -F(theta), with
+        // F = (sin(theta) - theta cos(theta)) / sin(theta)^3, taken from its Taylor series near the axis, where the quotient cancels.
+        // (The reference's acos(d.z) and 1 / sqrt(1 - d.z^2) lose all accuracy there and divide by zero where d.z rounds to 1.)
         V3 d = normalize(pt);
-        Real phi = atan2(d.y, d.x), r = acos(d.z) * 2 / Real(RB_PI);
-        Real dr = Real(-0.5) * (cos(phi) * dx + sin(phi) * dy), dphi = Real(0.5) * r * sin(phi) * dx - Real(0.5) * r * cos(phi) * dy;
-        Real dtheta = dr * (2 / Real(RB_PI));
-        Real q = d.x * d.x + d.y * d.y;
-        d_pt += d_normalize(pt, mk3(-dphi * d.y / q, dphi * d.x / q, -dtheta / sqrt(1 - d.z * d.z)));
+        Real rho = sqrt(d.x * d.x + d.y * d.y), theta = atan2(rho, d.z), t2 = theta * theta;
+        Real G = rho > 0 ? theta / rho : Real(1);
+        Real F = theta < Real(0.5) ? Real(1.0 / 3) + t2 * (Real(2.0 / 15) + t2 * (Real(2.0 / 63) + t2 * (Real(4.0 / 675) + t2 * (Real(2.0 / 2079) +
+                                                                                                                             t2 * Real(2764.0 / 19348875)))))
+                                   : (rho - theta * d.z) / (rho * rho * rho);
+        Real w = dx * d.x + dy * d.y;
+        d_pt += d_normalize(pt, mk3(-G * dx, -G * dy, w * F) * Real(1 / RB_PI));
         return;
     }
     if (cam.type == RB_CAMERA_PANORAMA) { // src/camera.h:698-724
+        // theta = atan2(rho, d.y), rho = sqrt(d.x^2 + d.z^2): its gradient (d.y d.x / rho, -rho, d.y d.z / rho) differs from the
+        // reference's (0, -1 / sqrt(1 - d.y^2), 0) by a radial part only, and stays accurate up to the poles.  At an exact pole the
+        // azimuth is undefined: both terms are dropped there, as the environment map's pole rule does.
         V3 d = normalize(pt);
         Real d_phi = dx / Real(2 * RB_PI), d_theta = dy / Real(RB_PI);
-        Real q = d.x * d.x + d.z * d.z;
-        d_pt += d_normalize(pt, mk3(-d_phi * d.z / q, -d_theta / sqrt(1 - d.y * d.y), d_phi * d.x / q));
+        Real q = d.x * d.x + d.z * d.z, rho = sqrt(q);
+        if (q > 0) d_pt += d_normalize(pt, mk3(-d_phi * d.z / q + d_theta * d.y * d.x / rho, -d_theta * rho, d_phi * d.x / q + d_theta * d.y * d.z / rho));
         return;
     }
     M3 K = cam_m3(cam.intr);

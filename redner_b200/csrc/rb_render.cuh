@@ -576,14 +576,8 @@ RB_D void bwd_sweep(const DevScene& sc, const KernelArgs& ka, int pixel, int px,
         d_envmap_eval(sc.env, ray.dir, rd, d_emission, ds.env_values, ds.env_w2e, d_ray.dir, d_footprint);
     }
     const Real delta = Real(1e-3);
-    Real psx = Real(0.5) / sc.cam.width, psy = Real(0.5) / sc.cam.height;
     DRay d_ray_dx, d_ray_dy;
-    d_ray_dx.org = d_prd.org_dx * (psx / delta);
-    d_ray_dx.dir = d_prd.dir_dx * (psx / delta);
-    d_ray_dy.org = d_prd.org_dy * (psy / delta);
-    d_ray_dy.dir = d_prd.dir_dy * (psy / delta);
-    d_ray.org += (d_prd.org_dx * (-psx) + d_prd.org_dy * (-psy)) / delta;
-    d_ray.dir += (d_prd.dir_dx * (-psx) + d_prd.dir_dy * (-psy)) / delta;
+    d_cam_primary_ray_diff(sc.cam, d_prd, d_ray, d_ray_dx, d_ray_dy);
     Sampler smp;
     smp.init(rp.sampler_type, rp.seed, pixel, (unsigned)s, sc.sobol_matrices, RB_SOBOL_BITS, (unsigned long long)s * main_draws_per_sample(sc, rp));
     double sx, sy;
@@ -723,7 +717,9 @@ RB_HD D2 d_cam_screen_to_camera_undistorted_d(const DevCamera& cam, D2 p, D3 d_d
         double d_cp = -d_dir.x * st, d_sp = -d_dir.y * st, d_st = -(d_dir.x * cp + d_dir.y * sp), d_ct = d_dir.z;
         double d_phi = d_sp * cp - d_cp * sp, d_theta = d_st * ct - d_ct * st;
         double d_r = d_theta * (pi / 2.0);
-        double d_x = d_phi * (-y / (x * x + y * y)) + d_r * (x / rr), d_y = d_phi * (x / (x * x + y * y)) + d_r * (y / rr);
+        // at the centre phi is atan2(0, 0) = 0 and d_phi / rr tends to -(pi / 2) d_dir.y: the limit of the two quotients below
+        double d_x = rr > 0 ? d_phi * (-y / (x * x + y * y)) + d_r * (x / rr) : d_r;
+        double d_y = rr > 0 ? d_phi * (x / (x * x + y * y)) + d_r * (y / rr) : -(pi / 2.0) * d_dir.y;
         r.x = d_x * 2;
         r.y = d_y * 2;
         return r;

@@ -458,6 +458,32 @@ class Scene:  # src/redner.cpp:62-73, src/scene.cpp:63-307
             raise RuntimeError("redner.Scene.light_sample_test: " + L.last_error(self._lib))
         return ints, doubles, pdfs
 
+    def camera_test(self, op, inputs, acc=None):
+        """Camera queries through the functions the render kernels call, on this scene's camera (rb_camera_test): test hook.  `op` is one
+        of _lib.RB_CAMTEST_*, `inputs` an [N, <= 64] float64 tensor on the scene's device (rows as in include/redner_b200.h, zero-padded).
+        `acc` is None or the [60, N] float32 accumulator the adjoint ops add to (query i's column is acc[:, i]; a camera without a lens
+        uses the first 58 rows); the adjoint ops get a zeroed one when it is None.  Returns ([N, 64] float64 outputs, acc)."""
+        import torch
+        inputs = inputs.to(torch.float64)
+        if inputs.dim() != 2 or inputs.shape[1] > 64:
+            raise ValueError("redner.Scene.camera_test: inputs must have shape [N, <= 64]")
+        n, dev = inputs.shape[0], inputs.device
+        rows = torch.zeros((n, 64), dtype=torch.float64, device=dev)
+        rows[:, :inputs.shape[1]] = inputs
+        out = torch.zeros((n, 64), dtype=torch.float64, device=dev)
+        if acc is None and op in (L.RB_CAMTEST_D_RAY, L.RB_CAMTEST_D_PROJECT):
+            acc = torch.zeros((60, n), dtype=torch.float32, device=dev)
+        if acc is not None and (acc.dtype != torch.float32 or not acc.is_contiguous() or tuple(acc.shape) != (60, n) or acc.device != dev):
+            raise ValueError("redner.Scene.camera_test: acc must be a contiguous float32 [60, N] tensor on the inputs' device")
+        stream = 0
+        if rows.is_cuda:
+            torch.cuda.set_device(dev)
+            stream = torch.cuda.current_stream(dev).cuda_stream
+        ptr = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None  # noqa: E731
+        if self._lib.rb_camera_test(self._handle, int(op), ptr(rows), n, ptr(out), ptr(acc), C.c_void_p(stream or 0)) != 0:
+            raise RuntimeError("redner.Scene.camera_test: " + L.last_error(self._lib))
+        return out, acc
+
     def last_stats(self):
         n = C.c_int(0)
         ms = C.c_float(0)

@@ -10,6 +10,7 @@
 #include <vector>
 
 #include "../../redner_b200/csrc/rb_render.cuh"
+#include "../../redner_b200/csrc/rb_camera_test.cuh"
 #include "../../redner_b200/csrc/rb_exact_layout.hpp"
 #include "../../redner_b200/csrc/rb_scene_host.hpp"
 
@@ -415,6 +416,23 @@ extern "C" int rb_light_sample_test(const rb_scene* sc, int light, const double*
     g_err = "rb_light_sample_test: this build has no emission textures";
     return 1;
 #endif
+}
+// Camera queries through the same camera_test_one as the library's hook, one query after another (host pointers).
+extern "C" int rb_camera_test(const rb_scene* sc, int op, const double* in, int n, double* out, float* acc, void*) {
+    const char* err = nullptr;
+    if (sc == nullptr) err = "null scene";
+    else if (sc->incomplete) err = "the scene's last update failed";
+    else if (op < RB_CAMTEST_CAMERA || op > RB_CAMTEST_FINISH) err = "unknown op";
+    else if (n < 0) err = "negative number of queries";
+    else if (n > 0 && (in == nullptr || out == nullptr)) err = "null buffer";
+    else if (n > 0 && acc == nullptr && (op == RB_CAMTEST_D_RAY || op == RB_CAMTEST_D_PROJECT))
+        err = "the adjoint ops need an accumulator";
+    if (err != nullptr) {
+        g_err = std::string("rb_camera_test: ") + err;
+        return 1;
+    }
+    for (long long i = 0; i < n; i++) camera_test_one(sc->dev.cam, op, in, n, out, acc, i);
+    return 0;
 }
 extern "C" int rb_scene_edge_list(const rb_scene* sc, int* num_edges, int* edges_out, size_t edges_bytes) {
     if (num_edges) *num_edges = sc->dev.num_edges;
