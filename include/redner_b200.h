@@ -463,6 +463,29 @@ enum {
 };
 int rb_camera_test(const rb_scene* scene, int op, const double* in, int n, double* out, float* acc, void* stream);
 
+/* Test hook: n geometry queries of one kind (`op`), one per thread, through the functions of rb_shape.cuh and the gradient scatters of
+ * rb_path.cuh that the render kernels call, on the shapes of a built scene.  in: [n, 96] doubles, out: [n, 96] doubles, one row per query;
+ * every row starts with the shape and triangle index (0, 1).  Inputs are rounded to float, as the kernels hold them.  A SurfacePoint is
+ * 35 numbers: position 0-2, geom_normal 3-5, shading frame x 6-8, y 9-11, n 12-14, dpdu 15-17, uv 18-19, du_dxy 20-21, dv_dxy 22-23,
+ * dn_dx 24-26, dn_dy 27-29, color 30-32, bary 33-34; a ray differential 12: org_dx, org_dy, dir_dx, dir_dy.  Rows (indices):
+ *   RB_SURFTEST_POINT    in: ray org 2-4, dir 5-7, differential 8-19.  out: tri_solve's u, v, t 0-2, u_dxy 3-4, v_dxy 5-6, t_dxy 7-8;
+ *                        make_surface_point's SurfacePoint 9-43 and rd_out 44-55; its decisions (0 / 1): the uv determinant is 0 56,
+ *                        the geometric normal flipped 57, the frame's y degenerate 58, coordinate_system's n.z < -1 + 1e-6 branch at
+ *                        the unflipped geometric normal 59 and at the shading normal 60; the uv determinant 61
+ *   RB_SURFTEST_D_POINT  in: the POINT inputs 2-19, d(SurfacePoint) 20-54, d(rd_out) 55-66.  out: d_make_surface_point's d_ray org 0-2,
+ *                        dir 3-5, d(ray differential) 6-17, d_vp 18-26, d_vn 27-35, d_vuv 36-41, d_vc 42-50 (per corner, zero-seeded);
+ *                        with d_shapes, scatter_vertex_grads adds them to the shape's gradient buffers
+ *   RB_SURFTEST_LIGHT    in: su 2, sv 3.  out: sample_light_triangle's position 0-2, geom_normal 3-5, frame x 6-8, y 9-11, n 12-14,
+ *                        bary 15-16, uv (the sample) 17-18; light_sample_uv 19-20; shape_tri_area 21
+ *   RB_SURFTEST_D_LIGHT  in: su 2, sv 3, d(position) 4-6, d(geom_normal) 7-9, d(frame x, y, n) 10-18, d(area) 19, d(uv) 20-21.
+ *                        out: d_sample_light_triangle's d_v 0-8, d_shape_tri_area's d_v 9-17; with d_shapes, d_light_sample_uv adds
+ *                        d(uv) to the shape's uv gradient
+ * d_shapes: NULL, or a host array of one rb_dshape per shape of the scene (device buffers, any may be NULL), scattered into with the
+ * kernels' warp-aggregated atomics.  `in` and `out` are memory of the scene's device.  An unknown op, a negative count, a shape or
+ * triangle index out of range, and the double-precision build are refused.  Runs on `stream` and synchronises it. */
+enum { RB_SURFTEST_POINT = 0, RB_SURFTEST_D_POINT = 1, RB_SURFTEST_LIGHT = 2, RB_SURFTEST_D_LIGHT = 3 };
+int rb_surface_test(const rb_scene* scene, int op, const double* in, int n, double* out, const rb_dshape* d_shapes, void* stream);
+
 const char* rb_last_error(void);
 const char* rb_version(void);
 

@@ -23,6 +23,8 @@ RB_TABLES = ("bvh_nodes", "bvh_triangles", "light_pmf", "light_cdf", "light_area
 RB_TRACE_ANY_HIT, RB_TRACE_BRUTE_FORCE = 1, 2
 # rb_camera_test ops (include/redner_b200.h)
 RB_CAMTEST_CAMERA, RB_CAMTEST_RAY, RB_CAMTEST_D_RAY, RB_CAMTEST_PROJECT, RB_CAMTEST_D_PROJECT, RB_CAMTEST_DISTORT, RB_CAMTEST_FINISH = range(7)
+# rb_surface_test ops (include/redner_b200.h)
+RB_SURFTEST_POINT, RB_SURFTEST_D_POINT, RB_SURFTEST_LIGHT, RB_SURFTEST_D_LIGHT = range(4)
 # int64 words per record of rb_render_exact / rb_exact_round: 10 limbs, then the counts of +inf, -inf and NaN contributions
 RB_EXACT_RECORD_WORDS = 13
 
@@ -137,7 +139,7 @@ class rb_dscene_desc(C.Structure):
 
 EXPORTS = [
     "rb_scene_create", "rb_scene_create_on_stream", "rb_scene_destroy", "rb_scene_max_generic_texture_dimension", "rb_compute_num_channels", "rb_render",
-    "rb_scene_set_partition", "rb_scene_last_stats", "rb_scene_last_stage_stats", "rb_scene_last_backward_stats", "rb_scene_last_live_samples", "rb_scene_last_exact_bytes", "rb_release_scratch", "rb_scene_build_ms", "rb_scene_edge_trees", "rb_scene_edge_list", "rb_scene_table", "rb_scene_trace_rays", "rb_exact_sum_test", "rb_texture_test", "rb_envmap_test", "rb_light_sample_test", "rb_camera_test", "rb_scene_set_camera", "rb_scene_update", "rb_render_batch", "rb_exact_record_count", "rb_render_exact", "rb_exact_round", "rb_last_error", "rb_version",
+    "rb_scene_set_partition", "rb_scene_last_stats", "rb_scene_last_stage_stats", "rb_scene_last_backward_stats", "rb_scene_last_live_samples", "rb_scene_last_exact_bytes", "rb_release_scratch", "rb_scene_build_ms", "rb_scene_edge_trees", "rb_scene_edge_list", "rb_scene_table", "rb_scene_trace_rays", "rb_exact_sum_test", "rb_texture_test", "rb_envmap_test", "rb_light_sample_test", "rb_camera_test", "rb_surface_test", "rb_scene_set_camera", "rb_scene_update", "rb_render_batch", "rb_exact_record_count", "rb_render_exact", "rb_exact_round", "rb_last_error", "rb_version",
 ]
 
 
@@ -214,6 +216,9 @@ def _bind(lib):
     if hasattr(lib, "rb_camera_test"):
         lib.rb_camera_test.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
         lib.rb_camera_test.restype = C.c_int
+    if hasattr(lib, "rb_surface_test"):
+        lib.rb_surface_test.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
+        lib.rb_surface_test.restype = C.c_int
     if hasattr(lib, "rb_exact_record_count"):
         lib.rb_exact_record_count.argtypes = [C.c_void_p, C.POINTER(rb_options), C.POINTER(rb_dscene_desc), C.c_void_p, C.POINTER(C.c_size_t),
                                               C.POINTER(C.c_uint64)]

@@ -178,6 +178,20 @@ RB_HD V2 tri_uv(const TriAttribs& a, Real u, Real v) {
     Real w = 1 - (u + v);
     return w * a.uv0 + u * a.uv1 + v * a.uv2;
 }
+// Determinant of the uv triangle's edge matrix as the reference computes it (src/shape.h:299-301): the float uv corners are subtracted in
+// double and the two products are rounded separately before their difference, never contracted into an FMA.  Two equal uv corners then
+// give two identical products and exactly 0, whatever the third corner is; a fused form leaves the rounding residual of one product
+// (about 1e-17 for uv0 = uv1 = (0.3, 0.7), uv2 = (0.01, 0.02)), and the dpdu branch flips.  make_surface_point and its adjoint both call
+// this, so they take the same branch.
+RB_HD double tri_uv_det(const TriAttribs& a) {
+    const double x02 = (double)a.uv0.x - a.uv2.x, y02 = (double)a.uv0.y - a.uv2.y, x12 = (double)a.uv1.x - a.uv2.x, y12 = (double)a.uv1.y - a.uv2.y;
+#ifdef __CUDA_ARCH__
+    return __dsub_rn(__dmul_rn(x02, y12), __dmul_rn(y02, x12));
+#else
+    volatile double p = x02 * y12, q = y02 * x12; // (host build: keep the compiler from contracting under -mfma / -ffp-contract=fast)
+    return p - q;
+#endif
+}
 RB_HD V3 shape_normal(const rb_shape& s, int i) {
     const float* p = s.normals + 3 * (size_t)i;
     return mk3(p[0], p[1], p[2]);
@@ -199,12 +213,12 @@ RB_HD SurfacePoint make_surface_point(const rb_shape& s, int tri, const Ray& ray
     p.position = mk3(rb_mul_add_unfused(ray.dir.x, t, ray.org.x), rb_mul_add_unfused(ray.dir.y, t, ray.org.y), rb_mul_add_unfused(ray.dir.z, t, ray.org.z));
     V3 gn = normalize(cross(v1 - v0, v2 - v0));
     V2 uv02 = a.uv0 - a.uv2, uv12 = a.uv1 - a.uv2;
-    Real det = uv02.x * uv12.y - uv02.y * uv12.x;
+    const double det = tri_uv_det(a);
     V3 dpdu = zero3(), dpdv = zero3();
     if (det == 0) {
         coordinate_system(gn, dpdu, dpdv);
     } else {
-        Real inv = 1 / det;
+        Real inv = 1 / (Real)det;
         V3 v02 = v0 - v2, v12 = v1 - v2;
         dpdu = (uv12.y * v02 - uv02.y * v12) * inv;
     }
@@ -221,8 +235,11 @@ RB_HD SurfacePoint make_surface_point(const rb_shape& s, int tri, const Ray& ray
         V3 dnn_dx = neg.x * n0 + h.u_dxy.x * n1 + h.v_dxy.x * n2;
         V3 dnn_dy = neg.y * n0 + h.u_dxy.y * n1 + h.v_dxy.y * n2;
         Real l2 = dot(nn, nn), l = sqrt(l2);
-        p.dn_dx = (l2 * dnn_dx - dot(nn, dnn_dx) * nn) / (l2 * l);
-        p.dn_dy = (l2 * dnn_dy - dot(nn, dnn_dy) * nn) / (l2 * l);
+        // (an interpolated normal of length 0 has no derivative: zero there instead of 0 / 0, as the adjoint skips it)
+        if (l2 * l > 0) {
+            p.dn_dx = (l2 * dnn_dx - dot(nn, dnn_dx) * nn) / (l2 * l);
+            p.dn_dy = (l2 * dnn_dy - dot(nn, dnn_dy) * nn) / (l2 * l);
+        }
         sn = normalize(nn);
         if (dot(gn, sn) < 0) gn = -gn;
     }
@@ -261,12 +278,12 @@ RB_HD void d_make_surface_point(const rb_shape& s, int tri, const Ray& ray, cons
     V3 ugn = cross(v1 - v0, v2 - v0);
     V3 gn = normalize(ugn);
     V2 uv02 = a.uv0 - a.uv2, uv12 = a.uv1 - a.uv2;
-    Real det = uv02.x * uv12.y - uv02.y * uv12.x;
+    const double det = tri_uv_det(a);
     V3 dpdu = zero3(), dpdv = zero3();
     if (det == 0) {
         coordinate_system(gn, dpdu, dpdv);
     } else {
-        Real inv = 1 / det;
+        Real inv = 1 / (Real)det;
         dpdu = (uv12.y * (v0 - v2) - uv02.y * (v1 - v2)) * inv;
     }
     V2 neg = -h.u_dxy - h.v_dxy;
@@ -390,7 +407,7 @@ RB_HD void d_make_surface_point(const rb_shape& s, int tri, const Ray& ray, cons
     if (det == 0) {
         d_coordinate_system(gn, d_dpdu, zero3(), d_gn);
     } else {
-        Real inv = 1 / det;
+        Real inv = 1 / (Real)det;
         V3 v02 = v0 - v2, v12 = v1 - v2;
         V2 d_uv02 = zero2(), d_uv12 = zero2();
         d_uv12.y += sum(d_dpdu * v02) * inv;

@@ -360,6 +360,7 @@ class Scene:  # src/redner.cpp:62-73, src/scene.cpp:63-307
         d = L.rb_scene_desc()
         d.camera = camera._c
         self._shapes = (L.rb_shape * max(1, len(shapes)))(*[s._c for s in shapes])
+        self._num_shapes = len(shapes)
         self._materials = (L.rb_material * max(1, len(materials)))(*[m._c for m in materials])
         self._lights = (L.rb_area_light * max(1, len(area_lights)))(*[a._c for a in area_lights])
         d.num_shapes, d.shapes = len(shapes), self._shapes
@@ -457,6 +458,39 @@ class Scene:  # src/redner.cpp:62-73, src/scene.cpp:63-307
                                           C.c_void_p(stream or 0)) != 0:
             raise RuntimeError("redner.Scene.light_sample_test: " + L.last_error(self._lib))
         return ints, doubles, pdfs
+
+    def surface_test(self, op, inputs, d_shapes=None):
+        """Geometry queries through the functions the render kernels call, on this scene's shapes (rb_surface_test): test hook.  `op` is
+        one of _lib.RB_SURFTEST_*, `inputs` an [N, <= 96] float64 tensor on the scene's device (rows as in include/redner_b200.h,
+        zero-padded).  `d_shapes` is None or one dict per shape of float32 gradient tensors ("vertices", "uvs", "normals", "colors", each
+        optional) that the adjoint ops scatter into.  Returns the [N, 96] float64 outputs."""
+        import torch
+        inputs = inputs.to(torch.float64)
+        if inputs.dim() != 2 or inputs.shape[1] > 96:
+            raise ValueError("redner.Scene.surface_test: inputs must have shape [N, <= 96]")
+        n, dev = inputs.shape[0], inputs.device
+        rows = torch.zeros((n, 96), dtype=torch.float64, device=dev)
+        rows[:, :inputs.shape[1]] = inputs
+        out = torch.zeros((n, 96), dtype=torch.float64, device=dev)
+        ptr = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None  # noqa: E731
+        dsh = None
+        if d_shapes is not None:
+            if len(d_shapes) != self._num_shapes:
+                raise ValueError("redner.Scene.surface_test: d_shapes needs one entry per shape of the scene (%d), not %d" % (self._num_shapes, len(d_shapes)))
+            for d in d_shapes:
+                for t in d.values():
+                    if t is not None and (t.dtype != torch.float32 or not t.is_contiguous() or t.device != dev):
+                        raise ValueError("redner.Scene.surface_test: gradient buffers must be contiguous float32 tensors on the inputs' device")
+            dsh = (L.rb_dshape * max(self._num_shapes, 1))()
+            for i, d in enumerate(d_shapes):
+                dsh[i] = L.rb_dshape(*(ptr(d.get(k)) for k in ("vertices", "uvs", "normals", "colors")))
+        stream = 0
+        if rows.is_cuda:
+            torch.cuda.set_device(dev)
+            stream = torch.cuda.current_stream(dev).cuda_stream
+        if self._lib.rb_surface_test(self._handle, int(op), ptr(rows), n, ptr(out), dsh, C.c_void_p(stream or 0)) != 0:
+            raise RuntimeError("redner.Scene.surface_test: " + L.last_error(self._lib))
+        return out
 
     def camera_test(self, op, inputs, acc=None):
         """Camera queries through the functions the render kernels call, on this scene's camera (rb_camera_test): test hook.  `op` is one

@@ -11,6 +11,7 @@
 
 #include "../../redner_b200/csrc/rb_render.cuh"
 #include "../../redner_b200/csrc/rb_camera_test.cuh"
+#include "../../redner_b200/csrc/rb_surface_test.cuh"
 #include "../../redner_b200/csrc/rb_exact_layout.hpp"
 #include "../../redner_b200/csrc/rb_scene_host.hpp"
 
@@ -432,6 +433,18 @@ extern "C" int rb_camera_test(const rb_scene* sc, int op, const double* in, int 
         return 1;
     }
     for (long long i = 0; i < n; i++) camera_test_one(sc->dev.cam, op, in, n, out, acc, i);
+    return 0;
+}
+// Geometry queries through the same surface_test_one as the library's hook, one query after another (host pointers).
+extern "C" int rb_surface_test(const rb_scene* sc, int op, const double* in, int n, double* out, const rb_dshape* d_shapes, void*) {
+    const char* err = n > 0 && out == nullptr ? "null buffer" : surface_test_check(sc, op, n, in, in);
+    if (err != nullptr) {
+        g_err = std::string("rb_surface_test: ") + err;
+        return 1;
+    }
+    DevDScene ds;
+    ds.shapes = d_shapes;
+    for (long long i = 0; i < n; i++) surface_test_one(sc->dev, d_shapes != nullptr ? &ds : nullptr, op, in, n, out, i);
     return 0;
 }
 extern "C" int rb_scene_edge_list(const rb_scene* sc, int* num_edges, int* edges_out, size_t edges_bytes) {
