@@ -5,8 +5,9 @@
 // All sets take the same arguments: the other translation units declare the same DevScene / KernelArgs layouts inside their
 // namespaces, so the driver's structs are passed to any of them as they are.
 #pragma once
+// prim_edge_project is null in the deterministic set, which projects every primary-edge sample itself.
 struct RenderKernels {
-    const void *forward, *bwd_trace, *bwd_sec_pick, *bwd_sec_shade, *bwd_sweep, *prim_keys, *primary_edge;
+    const void *forward, *bwd_trace, *bwd_sec_pick, *bwd_sec_shade, *bwd_sweep, *prim_keys, *primary_edge, *prim_edge_project;
 };
 RenderKernels render_kernels();
 namespace rb_lean {

@@ -6,7 +6,8 @@
 //   forward    k_forward / k_forward_channels   camera sample -> primary hit -> emission -> bounce loop -> pixel
 //   backward   per band of samples:  k_bwd_trace (primal replay, records, work lists by warp ballot) -> k_bwd_sec_pick ->
 //              counting sort by edge (k_sec_offsets, k_sec_scatter) -> k_bwd_sec_shade (boundary terms) -> k_bwd_sweep (reverse
-//              sweep, first-hit and camera adjoints);  then k_prim_keys -> radix sort -> k_primary_edge;  k_finish_camera
+//              sweep, first-hit and camera adjoints);  then k_prim_keys -> radix sort -> k_primary_edge per band of edge samples,
+//              k_prim_edge_project;  k_finish_camera
 // Every kernel is small enough for the GPC instruction cache and walks the stages of a sample block-synchronously
 // (RB_PHASE_SYNC): a fused megakernel of the same code ran instruction-fetch bound at 6 % issue utilisation.
 // Forward: a warp owns 32/L pixels with L lanes per pixel (L = min(32, 2^floor(log2 spp))); lanes of a pixel are its
@@ -221,8 +222,12 @@ static int render_pass(const rb_scene* scene_, const rb_options* opt, float* ima
             ka.screen_grad = xl.screen_grad;
         }
         int n_cam = cam_acc_count(cam);
+        // Without a lens the default sets sum each edge's screen-space adjoints and project them once per edge (k_prim_edge_project):
+        // k_primary_edge then needs no camera columns in shared memory.
+        const bool primary = primary_edge_pass_runs(scene->dev);
+        const bool per_edge = primary && !det && !RB_CAM_LENS(cam);
         const size_t cam_smem_sweep = det ? RB_SMEM_CAM_EXACT(n_cam) : RB_SMEM_CAM(n_cam, RB_BLOCK_SWEEP),
-                     cam_smem_prim = det ? RB_SMEM_CAM_EXACT(n_cam) : RB_SMEM_CAM(n_cam, RB_BLOCK_PRIM);
+                     cam_smem_prim = det ? RB_SMEM_CAM_EXACT(n_cam) : per_edge ? 0 : RB_SMEM_CAM(n_cam, RB_BLOCK_PRIM);
         const long long exact_max_samples = exact_band_samples(rp.max_bounces);
         if (det && exact_max_samples < 1) {
             rb_set_error("rb_render: deterministic mode supports at most 2097150 bounces");
@@ -253,7 +258,6 @@ static int render_pass(const rb_scene* scene_, const rb_options* opt, float* ima
         // boundary terms: vertex list, edge picks, (edge, vertex) per slot, slots in edge order
         const size_t vert_cap = (size_t)band * ka.rec_per_sample, slots = vert_cap + 32;
         ka.vert_cap = (int)vert_cap;
-        const bool primary = primary_edge_pass_runs(scene->dev);
         const long long n_px_all = (long long)rp.vp_w * rp.vp_h;
         const long long total_e = primary ? ((n_px_all - rp.part + rp.num_parts - 1) / rp.num_parts) * rp.spp : 0; // i % num_parts == part
         const long long band_e = std::min<long long>(std::max<long long>(total_e, 1), det ? std::min(1LL << 26, exact_max_samples) : 1LL << 26);
@@ -261,8 +265,8 @@ static int render_pass(const rb_scene* scene_, const rb_options* opt, float* ima
         cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, (const unsigned*)nullptr, (unsigned*)nullptr, (const unsigned*)nullptr, (unsigned*)nullptr, (int)band_e, 0, 32, stream);
 
         // ---- scratch layout, in carving order, every buffer 256-byte aligned: gradient descriptors | camera accumulators | band counters |
-        //      edge histogram, offsets and cursors | live-pixel list, its count and its selection temporaries | band (records, boundary
-        //      terms, work lists).  The primary-edge pass runs after the
+        //      edge histogram | per-edge primary-edge adjoint sums | edge offsets and cursors | live-pixel list, its count and its selection
+        //      temporaries | band (records, boundary terms, work lists).  The primary-edge pass runs after the
         //      bands and reuses the band area for its keys / values (double buffers) and radix-sort temporaries.  The buffers of the
         //      boundary stage are empty when it does not run.  carve(nullptr) only measures; both calls return the size.
         rb_dshape* d_shapes;
@@ -293,11 +297,14 @@ static int render_pass(const rb_scene* scene_, const rb_options* opt, float* ima
             exact_acc = (long long*)take(det ? (size_t)(xl.num_acc + 1) * RB_EXACT_WORDS * sizeof(long long) : 0);
             exact_ranges = (ExactRange*)take(det ? std::max<size_t>(xl.ranges.size(), 1) * sizeof(ExactRange) : 0);
             exact_rec_first = (long long*)take(xo ? std::max<size_t>(xl.rec_first.size(), 1) * sizeof(long long) : 0);
-            // Every pass starts with these three at zero.  They stay adjacent, carved one after the other, so that one memset clears them.
+            // Every pass starts with these four at zero.  They stay adjacent, carved one after the other, so that one memset clears them.
+            // The per-edge sums span every primary-edge band, outside the band area that the keys and values reuse.
             const size_t zeroed_begin = off;
             cam_accum = (double*)take(RB_CAM_ACC_LENS * sizeof(double));
             counters = (BandCounters*)take((size_t)max_bands * sizeof(BandCounters));
             ka.edge_hist = (unsigned*)take(secondary ? n_edges * 4 : 0);
+            double* edge_adj = (double*)take(per_edge ? n_edges * 4 * sizeof(double) : 0);
+            ka.edge_adj = per_edge ? edge_adj : nullptr;
             zeroed_bytes = off - zeroed_begin;
             ka.edge_offs = (unsigned*)take(secondary ? n_edges * 4 : 0);
             ka.edge_cursor = (unsigned*)take(secondary ? n_edges * 4 : 0);
@@ -360,7 +367,7 @@ static int render_pass(const rb_scene* scene_, const rb_options* opt, float* ima
         long long n_acc = xl.num_acc;
         void* normalise_args[] = {&exact_acc, &n_acc};
         const int grid_x = sms * 4;
-        RB_CUDA_OK(cudaMemsetAsync(cam_accum, 0, zeroed_bytes, stream)); // camera accumulators, band counters, edge histogram
+        RB_CUDA_OK(cudaMemsetAsync(cam_accum, 0, zeroed_bytes, stream)); // camera accumulators, band counters, edge histogram, edge sums
         ka.ds.shapes = d_shapes;
         ka.ds.materials = d_mats;
         ka.ds.light_intensity = d_lights;
@@ -443,6 +450,10 @@ static int render_pass(const rb_scene* scene_, const rb_options* opt, float* ima
                     RB_CUDA_OK(cudaLaunchKernel(xk.normalise, grid_x, 256, normalise_args, 0, stream));
                     launches++;
                 }
+            }
+            if (per_edge) {
+                RB_CUDA_OK(cudaLaunchKernel(bkern.prim_edge_project, (scene->dev.num_edges + RB_BLOCK_PRIM - 1) / RB_BLOCK_PRIM, RB_BLOCK_PRIM, args, 0, stream));
+                launches++;
             }
         }
         RB_CUDA_OK(cudaEventRecord(ev[EV_AFTER_PRIMARY_EDGE], stream));

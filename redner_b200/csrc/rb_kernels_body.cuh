@@ -473,6 +473,41 @@ __global__ void __launch_bounds__(256) k_prim_keys(const __grid_constant__ DevSc
         vals[t] = (unsigned)t;
     }
 }
+#ifndef RB_DETERMINISTIC
+// Adds a thread's run of primary-edge adjoints (the sums s[0..3] of edge e's samples) to the edge's sums in edge_adj.  The lanes of the
+// current convergence group that flush the same edge are added together first (pointer doubling, as in warp_agg_add3) and the group
+// leader issues the reductions.  Must stay inline for the same reason as warp_agg_add3.
+RB_D void flush_edge_adjoint(double* edge_adj, int e, double s0, double s1, double s2, double s3) {
+    unsigned peers = __match_any_sync(__activemask(), e);
+    int lane = threadIdx.x & 31;
+    unsigned above = peers & (0xfffffffeu << lane);
+    int nxt = above ? __ffs(above) - 1 : -1;
+    int n = __popc(peers);
+#pragma unroll 1
+    for (int span = 1; span < n; span <<= 1) {
+        int src = nxt >= 0 ? nxt : lane;
+        double o0 = __shfl_sync(peers, s0, src), o1 = __shfl_sync(peers, s1, src), o2 = __shfl_sync(peers, s2, src), o3 = __shfl_sync(peers, s3, src);
+        int nn = __shfl_sync(peers, nxt, src);
+        if (nxt >= 0) {
+            s0 += o0; s1 += o1; s2 += o2; s3 += o3;
+            nxt = nn;
+        }
+    }
+    if (lane == __ffs(peers) - 1) {
+        double* a = edge_adj + 4 * (size_t)e;
+        if (s0 != 0) atomicAdd(a + 0, s0);
+        if (s1 != 0) atomicAdd(a + 1, s1);
+        if (s2 != 0) atomicAdd(a + 2, s2);
+        if (s3 != 0) atomicAdd(a + 3, s3);
+    }
+}
+#endif
+// Shades the band's primary-edge samples in key order.  The deterministic instantiation and a camera with a lens project every sample
+// (primary_edge_sample), the camera's gradients in per-thread shared-memory columns.  Otherwise the projection is linear in the
+// screen-space adjoints and fixed per edge: each thread sums the adjoints of its run of samples of one edge in double, adds the run to
+// ka.edge_adj when the edge changes, and k_prim_edge_project projects each edge's sum once.  The sort puts the samples of one edge next to
+// each other, so a thread meets few edges (at most three on C2) and every lane of a warp mostly flushes the same one.  That path launches
+// with no dynamic shared memory.
 __global__ void __launch_bounds__(RB_BLOCK_PRIM, RB_MIN_BLOCKS_PRIM) k_primary_edge(const __grid_constant__ DevScene sc, const __grid_constant__ KernelArgs ka, int dim_base,
                                                                                long long t0, int n, const unsigned* keys, const unsigned* vals) {
     const int n_cam = cam_acc_count(sc.cam);
@@ -481,13 +516,6 @@ __global__ void __launch_bounds__(RB_BLOCK_PRIM, RB_MIN_BLOCKS_PRIM) k_primary_e
     exact_camera_begin(cam_exact, n_cam);
     CamAcc cam_acc;
     cam_acc.exact = cam_exact;
-#else
-    extern __shared__ float cam_smem[]; // [n_cam][blockDim.x]
-    for (int k = 0; k < n_cam; k++) cam_smem[k * blockDim.x + threadIdx.x] = 0.f;
-    CamAcc cam_acc;
-    cam_acc.base = cam_smem + threadIdx.x;
-    cam_acc.stride = blockDim.x;
-#endif
     RB_BLOCK_LOOP(t, n) {
         RB_PRIM_SYNC();
         if (t < n && keys[t] != 0xffffffffu) {
@@ -497,12 +525,60 @@ __global__ void __launch_bounds__(RB_BLOCK_PRIM, RB_MIN_BLOCKS_PRIM) k_primary_e
             primary_edge_sample(sc, ka, i, s, dim_base, cam_acc);
         }
     }
-#ifdef RB_DETERMINISTIC
     exact_camera_flush(cam_exact, n_cam);
 #else
-    block_reduce_camera(cam_smem, ka.ds.cam_accum, n_cam);
+    const bool lens = RB_CAM_LENS(sc.cam); // (block-uniform; always false in the sets without lenses)
+    extern __shared__ float cam_smem[];   // [n_cam][blockDim.x], with a lens only
+    CamAcc cam_acc;
+    cam_acc.base = cam_smem + threadIdx.x;
+    cam_acc.stride = blockDim.x;
+    if (lens)
+        for (int k = 0; k < n_cam; k++) cam_smem[k * blockDim.x + threadIdx.x] = 0.f;
+    int run_e = -1; // the edge of this thread's run, and its sums
+    double r0 = 0, r1 = 0, r2 = 0, r3 = 0;
+    RB_BLOCK_LOOP(t, n) {
+        RB_PRIM_SYNC();
+        PrimEdgeAdjoint a;
+        bool hit = false;
+        if (t < n && keys[t] != 0xffffffffu) {
+            long long i;
+            int s;
+            prim_sample_id(ka.rp, t0 + vals[t], i, s);
+            hit = primary_edge_screen_adjoint(sc, ka, i, s, dim_base, a);
+        }
+        if (hit && lens) primary_edge_project(sc, ka, a.edge_id, a.lu, a.d0x, a.d0y, a.d1x, a.d1y, cam_acc);
+        else if (hit) {
+            if (a.edge_id != run_e) {
+                if (run_e >= 0) flush_edge_adjoint(ka.edge_adj, run_e, r0, r1, r2, r3);
+                run_e = a.edge_id;
+                r0 = r1 = r2 = r3 = 0;
+            }
+            r0 += a.d0x; r1 += a.d0y;
+            r2 += a.d1x; r3 += a.d1y;
+        }
+    }
+    if (run_e >= 0) flush_edge_adjoint(ka.edge_adj, run_e, r0, r1, r2, r3);
+    if (lens) block_reduce_camera(cam_smem, ka.ds.cam_accum, n_cam);
 #endif
 }
+#ifndef RB_DETERMINISTIC
+// After the last primary-edge band: one thread per edge projects the edge's summed screen-space adjoints (edge_adj) into its vertices'
+// gradients and the camera accumulators, exactly as primary_edge_project does for one sample.  Edges no sample contributed to are skipped.
+__global__ void __launch_bounds__(RB_BLOCK_PRIM) k_prim_edge_project(const __grid_constant__ DevScene sc, const __grid_constant__ KernelArgs ka) {
+    __shared__ float cam_smem[RB_CAM_ACC * RB_BLOCK_PRIM]; // [RB_CAM_ACC][blockDim.x]
+    for (int k = 0; k < RB_CAM_ACC; k++) cam_smem[k * blockDim.x + threadIdx.x] = 0.f;
+    CamAcc cam_acc;
+    cam_acc.base = cam_smem + threadIdx.x;
+    cam_acc.stride = blockDim.x;
+    const int e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e < sc.num_edges) {
+        const double* a = ka.edge_adj + 4 * (size_t)e;
+        const double s0 = a[0], s1 = a[1], s2 = a[2], s3 = a[3];
+        if (s0 != 0 || s1 != 0 || s2 != 0 || s3 != 0) primary_edge_project(sc, ka, e, d2(0, 0), (Real)s0, (Real)s1, (Real)s2, (Real)s3, cam_acc);
+    }
+    block_reduce_camera(cam_smem, ka.ds.cam_accum, RB_CAM_ACC);
+}
+#endif
 
 // The kernels of this instantiation that rb_render launches through a RenderKernels table (rb_kernel_set.h).
 RenderKernels render_kernels() {
@@ -514,6 +590,11 @@ RenderKernels render_kernels() {
     k.bwd_sweep = (const void*)k_bwd_sweep;
     k.prim_keys = (const void*)k_prim_keys;
     k.primary_edge = (const void*)k_primary_edge;
+#ifdef RB_DETERMINISTIC
+    k.prim_edge_project = nullptr;
+#else
+    k.prim_edge_project = (const void*)k_prim_edge_project;
+#endif
     return k;
 }
 

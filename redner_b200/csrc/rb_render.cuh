@@ -51,6 +51,7 @@ struct KernelArgs {
     unsigned *sec_keys, *sec_vals; // [slot] picked edge (or 0xffffffff) / vert_list entry
     unsigned *edge_hist, *edge_offs, *edge_cursor; // [num_edges] counting sort of the picks by edge
     unsigned* sec_order;         // [picks] slots in edge order
+    double* edge_adj;            // [num_edges][4] primary-edge screen-space adjoints summed per edge (k_primary_edge without a lens), or null
 };
 
 RB_HD int rb_channel_width(int ch, int max_generic) { // floats of one channel, src/channels.cpp:42-113
@@ -931,19 +932,26 @@ RB_D void filter_splat(const DevCamera& cam, const RenderParams& rp, const float
         }
     }
 }
-RB_D void primary_edge_sample(const DevScene& sc, const KernelArgs& ka, long long i, int s, int dim_base, CamAcc& cam_acc) {
+// What one primary-edge sample hands to the projection: its edge, its lens point and the screen-space adjoints of the edge's two
+// projected end points.
+struct PrimEdgeAdjoint {
+    int edge_id;
+    D2 lu;
+    Real d0x, d0y, d1x, d1y;
+};
+// The per-sample part of a primary-edge sample: the pick, the two edge rays, the contribution, and the screen_grad scatter.  False when the
+// sample adds nothing; otherwise `a` holds the adjoints that primary_edge_project turns into vertex and camera gradients.
+RB_D bool primary_edge_screen_adjoint(const DevScene& sc, const KernelArgs& ka, long long i, int s, int dim_base, PrimEdgeAdjoint& a) {
     const RenderParams& rp = ka.rp;
-    const DevDScene& ds = ka.ds;
     const Real weight = Real(1) / Real(rp.spp);
     Sampler smp;
     PrimEdgePick pk;
-    if (!primary_edge_pick(sc, rp, i, s, dim_base, smp, pk)) return;
+    if (!primary_edge_pick(sc, rp, i, s, dim_base, smp, pk)) return false;
     const D2 lu = pick_lens(pk);
-    if (ka.zero_cull && edge_point_adjoint_is_zero(sc, ka, pk.ept)) return; // (before any ray: k_prim_keys drops these samples too)
+    if (ka.zero_cull && edge_point_adjoint_is_zero(sc, ka, pk.ept)) return false; // (before any ray: k_prim_keys drops these samples too)
     const double pmf = pk.pmf;
     const D2 q0 = pk.q0, q1 = pk.q1, ept = pk.ept;
     const Edge edge = sc.edges[pk.edge_id];
-    V3 v0 = edge_v0(sc.shapes, edge), v1 = edge_v1(sc.shapes, edge);
     int vp_w = rp.vp_w;
     int xi, yi;
     edge_point_pixel(sc.cam, ept, xi, yi);
@@ -976,7 +984,7 @@ RB_D void primary_edge_sample(const DevScene& sc, const KernelArgs& ka, long lon
         // (primary_edge_weights_updater, src/edge.cpp:653-676)
         connected = connected || (hits[side].shape_id == edge.shape_id && (hits[side].tri_id == edge.f0 || hits[side].tri_id == edge.f1));
     }
-    if (!connected) return;
+    if (!connected) return false;
     for (int side = 0; side < 2; side++) {
         const Ray ray = rays[side];
         const Isect is = hits[side];
@@ -1011,7 +1019,7 @@ RB_D void primary_edge_sample(const DevScene& sc, const KernelArgs& ka, long lon
             contrib += (side == 0 ? weight : -weight) * acc * (Real)(pk.jacobian / pmf);
         }
     }
-    if (contrib == 0) return;
+    if (contrib == 0) return false;
     // gradients of the edge equation w.r.t. the projected end points and the edge point
     Real d0x, d0y, d1x, d1y, dex, dey;
     if (cam_is_linear(sc.cam)) { // Eq. 8
@@ -1025,19 +1033,35 @@ RB_D void primary_edge_sample(const DevScene& sc, const KernelArgs& ka, long lon
         d1x = (Real)g[2] * contrib; d1y = (Real)g[3] * contrib;
         dex = (Real)g[4] * contrib; dey = (Real)g[5] * contrib;
     }
-    V3 d_v0 = zero3(), d_v1 = zero3();
-    if (RB_CAM_LENS(sc.cam)) d_cam_project_lens(sc.cam, v0, v1, lu, d0x, d0y, d1x, d1y, cam_acc, d_v0, d_v1);
-    else d_cam_project(sc.cam, v0, v1, d0x, d0y, d1x, d1y, cam_acc, d_v0, d_v1);
-    float* dv = ds.shapes[edge.shape_id].vertices;
-    if (dv) {
-        agg_add3(dv + 3 * (size_t)edge.v0, d_v0);
-        agg_add3(dv + 3 * (size_t)edge.v1, d_v1);
-    }
     if (ka.screen_grad) {
         size_t pix = (size_t)yi * vp_w + xi;
         rb_red_add(&ka.screen_grad[2 * pix + 0], (float)dex);
         rb_red_add(&ka.screen_grad[2 * pix + 1], (float)dey);
     }
+    a.edge_id = pk.edge_id;
+    a.lu = lu;
+    a.d0x = d0x; a.d0y = d0y;
+    a.d1x = d1x; a.d1y = d1y;
+    return true;
+}
+// The projection of a primary-edge sample: the adjoints (d0x, d0y, d1x, d1y) of edge `edge_id`'s projected end points, through the camera
+// projection, into its two vertices' gradients and the camera accumulators.  Linear in the adjoints, and apart from the lens point it
+// depends on the edge alone, so without a lens k_primary_edge runs it once per edge on the sum of the edge's samples (k_prim_edge_project).
+RB_D void primary_edge_project(const DevScene& sc, const KernelArgs& ka, int edge_id, D2 lu, Real d0x, Real d0y, Real d1x, Real d1y, CamAcc& cam_acc) {
+    const Edge edge = sc.edges[edge_id];
+    V3 v0 = edge_v0(sc.shapes, edge), v1 = edge_v1(sc.shapes, edge);
+    V3 d_v0 = zero3(), d_v1 = zero3();
+    if (RB_CAM_LENS(sc.cam)) d_cam_project_lens(sc.cam, v0, v1, lu, d0x, d0y, d1x, d1y, cam_acc, d_v0, d_v1);
+    else d_cam_project(sc.cam, v0, v1, d0x, d0y, d1x, d1y, cam_acc, d_v0, d_v1);
+    float* dv = ka.ds.shapes[edge.shape_id].vertices;
+    if (dv) {
+        agg_add3(dv + 3 * (size_t)edge.v0, d_v0);
+        agg_add3(dv + 3 * (size_t)edge.v1, d_v1);
+    }
+}
+RB_D void primary_edge_sample(const DevScene& sc, const KernelArgs& ka, long long i, int s, int dim_base, CamAcc& cam_acc) {
+    PrimEdgeAdjoint a;
+    if (primary_edge_screen_adjoint(sc, ka, i, s, dim_base, a)) primary_edge_project(sc, ka, a.edge_id, a.lu, a.d0x, a.d0y, a.d1x, a.d1y, cam_acc);
 }
 
 // Turns the reduced matrix gradients into the user-facing camera gradients (everything is linear in the accumulated

@@ -22,7 +22,7 @@ import tempfile
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 TUS = {"lean": "rb_kernels_lean.cu", "diffuse": "rb_kernels_diffuse.cu", "general": "rb_kernels.cu", "det": "rb_kernels_det.cu"}
-HOT = ["k_forward", "k_bwd_trace", "k_bwd_sec_pick", "k_bwd_sec_shade", "k_bwd_sweep", "k_primary_edge"]
+HOT = ["k_forward", "k_bwd_trace", "k_bwd_sec_pick", "k_bwd_sec_shade", "k_bwd_sweep", "k_primary_edge", "k_prim_edge_project"]
 TEX_FUNCS = ["bilerp_tap", "bilerp_eval", "tex_level", "tex_eval_mip", "tex_eval", "mat_diffuse", "mat_specular", "mat_roughness",
              "mat_normal_tex"]
 
